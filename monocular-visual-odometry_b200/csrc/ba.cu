@@ -79,8 +79,9 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
-// exp of a g2o SE3 update (omega, upsilon) applied on the left of (R, t): out = exp(d) * in
-__device__ void se3_update(const double *d, const double *in, double *out) {
+// exp of a g2o SE3 update (omega, upsilon) applied on the left of (R, t): out = exp(d) * in.  Inlined: as a call its d[]
+// argument went through the stack.
+__device__ __forceinline__ void se3_update(const double *d, const double *in, double *out) {
   const double wx = d[0], wy = d[1], wz = d[2];
   const double th2 = wx * wx + wy * wy + wz * wz;
   double a, b, c;
@@ -563,7 +564,8 @@ size_t ba_smem_doubles(int F, int nact, int pc) {
 // then across the 8 CTAs through distributed shared memory (every CTA reads all partials in rank
 // order, so all CTAs hold identical state and decide identically).  The pass that evaluates a trial
 // step also linearises at the trial point, so an accepted step needs no second pass: one pass and
-// one cluster barrier per LM trial.
+// one cluster barrier per LM trial.  Per trial: solve (lane 0 of warp f for frame f) -> CTA barrier ->
+// pass -> CTA barrier -> cross-warp sum -> cluster barrier -> gather + decision (warp-local, no CTA barrier).
 #ifndef MVO_PF_T
 #define MVO_PF_T 512
 #endif
@@ -665,7 +667,8 @@ __device__ __forceinline__ void edge_terms(const PoseArgs &a, const double *Rt, 
     rho = 2 * (chi * ys) * a.huber - a.huber * a.huber;
   }
   v[27] += rho;
-  // EdgeProjectXYZ2UV::linearizeOplus, pose block (rows scaled by fx / fy)
+  // EdgeProjectXYZ2UV::linearizeOplus, pose block (rows scaled by fx / fy).  B[4] and B[9] are structural zeros; the
+  // products with them stay (DESIGN.md §8, tried and rejected: leaving them out changes the rounding of the sums).
   const double fxz = a.fx * iz, fyz = a.fy * iz;
   const double B[12] = {xz * yz * a.fx, -(1 + xz * xz) * a.fx, yz * a.fx, -fxz, 0, xz * fxz,
                         (1 + yz * yz) * a.fy, -xz * yz * a.fy, -xz * a.fy, 0, -fyz, yz * fyz};
@@ -683,19 +686,28 @@ __device__ __forceinline__ void edge_terms(const PoseArgs &a, const double *Rt, 
   for (int r = 0; r < 6; ++r) v[21 + r] += B[r] * r0 + B[6 + r] * r1;
 }
 
+// One halving step of warp_fold32: lanes with bit STEP set keep the upper half, the others the lower half.  STEP is a template
+// argument so that the loop has a constant trip count before any unrolling: with a bound taken from an enclosing loop's variable
+// the front end left the loop rolled and demoted v[] to local memory (every access of the fold an LDL / STL).
+template <int STEP>
+__device__ __forceinline__ void warp_fold_step(double (&v)[32], int lane) {
+  const bool up = (lane & STEP) != 0;
+#pragma unroll
+  for (int i = 0; i < STEP; ++i) {
+    const double send = up ? v[i] : v[i + STEP];
+    const double keep = up ? v[i + STEP] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, STEP);
+  }
+}
+
 // warp reduce-scatter of 32 values: afterwards lane L holds the warp-wide sum of v[L]
 // (31 exchanges instead of 32 x 5 for a butterfly per value)
 __device__ __forceinline__ double warp_fold32(double (&v)[32], int lane) {
-#pragma unroll
-  for (int step = 16; step >= 1; step >>= 1) {
-    const bool up = (lane & step) != 0;
-#pragma unroll
-    for (int i = 0; i < step; ++i) {
-      const double send = up ? v[i] : v[i + step];
-      const double keep = up ? v[i + step] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, step);
-    }
-  }
+  warp_fold_step<16>(v, lane);
+  warp_fold_step<8>(v, lane);
+  warp_fold_step<4>(v, lane);
+  warp_fold_step<2>(v, lane);
+  warp_fold_step<1>(v, lane);
   return v[0];
 }
 
@@ -788,14 +800,14 @@ template <int CH, bool CACHED, bool STORE>
 __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), csize = cluster.num_blocks();
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   pdl_wait();                                // PnP finish / the glue kernel wrote what this kernel reads (launch_pdl.cuh)
   pdl_launch_dependents();
   extern __shared__ __align__(16) double sm[];
   __shared__ int s_ef[PF_T];
   __shared__ double s_c[8];                  // 0 lambda, 2 chi (initial)
-  __shared__ double s_fscale[BA_MAXF], s_fstep[BA_MAXF];
-  __shared__ int s_okf[BA_MAXF];
+  __shared__ double s_fscale[2][BA_MAXF], s_fstep[2][BA_MAXF];     // by trial parity: a solve never overwrites what a
+  __shared__ int s_okf[2][BA_MAXF];                                // slower warp is still reading for the previous decision
   __shared__ int s_fslot[BA_MAXF], s_fcnt[BA_MAXF], s_cstart[BA_MAXF + 1], s_F;
   int F = a.F, nchunks = CACHED ? a.E / CH : a.E / a.chunk;
   if (STORE) {
@@ -879,25 +891,40 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
   }
   __syncthreads();
   int parity = 0;
-  auto gather = [&](double *dst) {           // after the barrier: sum the partials of all CTAs in rank order
-    double *mine = parity ? s_part1 : s_part0;
+  // After the cluster barrier: sum the partials of all CTAs in rank order.  Warp w writes the rows of frames w, w + PF_NW, ..
+  // of dst, which only that warp's lane 0 reads (the solve of those frames), so no CTA barrier follows.  Every warp also sums
+  // the chi2 of each frame into lane f, the same sum as dst[f * PF_V + 27]: the LM decision is taken from registers.
+  auto gather = [&](double *dst) -> double {
+    const double *mine = parity ? s_part1 : s_part0;
+    auto sum_ranks = [&](int i, int j, double &si, double &sj) {      // elements i and j (-1: none), all loads in flight together
+      double v[PF_MAXC], u[PF_MAXC];
+#pragma unroll
+      for (unsigned r = 0; r < PF_MAXC; ++r) {
+        v[r] = r < csize && i >= 0 ? *cluster.map_shared_rank(mine + i, r) : 0.0;
+        u[r] = r < csize && j >= 0 ? *cluster.map_shared_rank(mine + j, r) : 0.0;
+      }
+      si = 0; sj = 0;
+#pragma unroll
+      for (unsigned r = 0; r < PF_MAXC; ++r) { si += v[r]; sj += u[r]; }       // fixed rank order: identical in every CTA
+    };
     cluster.sync();
-    for (int i = tid; i < NV; i += PF_T) {
-      double v[PF_MAXC];
-#pragma unroll
-      for (unsigned r = 0; r < PF_MAXC; ++r) v[r] = r < csize ? *cluster.map_shared_rank(mine + i, r) : 0.0;
-      double s2 = 0;
-#pragma unroll
-      for (unsigned r = 0; r < PF_MAXC; ++r) s2 += v[r];        // fixed rank order: identical in every CTA
-      dst[i] = s2;
+    double chi_f, row, unused;
+    if (warp < F) {                                                 // warp-uniform: the other warps issue only the chi2 loads
+      sum_ranks(lane < F ? lane * PF_V + 27 : -1, lane < PF_V ? warp * PF_V + lane : -1, chi_f, row);
+      if (lane < PF_V) dst[warp * PF_V + lane] = row;
+    } else {
+      sum_ranks(lane < F ? lane * PF_V + 27 : -1, -1, chi_f, unused);
     }
+    for (int f = warp + PF_NW; f < F; f += PF_NW)                   // only when PF_NW < F
+      if (lane < PF_V) { sum_ranks(f * PF_V + lane, -1, row, unused); dst[f * PF_V + lane] = row; }
     parity ^= 1;
-    __syncthreads();
+    return chi_f;
   };
   double *s_cur = s_lin0, *s_new = s_lin1;
   double *p_cur = s_pose, *p_try = s_try;    // poses ping-pong like the linearisations
   pose_pass<CH, CACHED>(a, F, nchunks, p_cur, s_ed, s_ef, s_wacc, parity ? s_part1 : s_part0, rank, csize);
   gather(s_cur);
+  __syncthreads();                           // the initial chi2 and damping below read every frame's rows
   if (STORE) {                               // behind the cluster barrier of the gather: out_info[1] has been zeroed
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) my_edges += __shfl_xor_sync(0xffffffffu, my_edges, o);
@@ -929,9 +956,12 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
     bool accepted = false, tiny = false;
     double mstep = 0;
     do {
-      // per-frame 6x6 solve + trial pose + this frame's share of the gain denominator (every CTA, identically)
-      if (tid < F) {
-        const int f = tid;
+      // per-frame 6x6 solve + trial pose + this frame's share of the gain denominator (every CTA, identically), on lane 0 of
+      // the warp that gathered the frame's rows
+      const int b = trials & 1;
+      __syncwarp();
+      for (int f = warp; f < F; f += PF_NW) {
+        if (lane != 0) continue;
         double d[6] = {0, 0, 0, 0, 0, 0};
         bool ok = true;
         const bool fixed = a.fix_first && f == 0;
@@ -945,15 +975,15 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
         if (ok && !fixed)
 #pragma unroll
           for (int q = 0; q < 6; ++q) { sc += d[q] * (lambda * d[q] + s_cur[f * PF_V + 21 + q]); ms = fmax(ms, fabs(d[q])); }   // computeScale, CURRENT b
-        s_fscale[f] = sc;
-        s_fstep[f] = ms;
-        s_okf[f] = ok;
+        s_fscale[b][f] = sc;
+        s_fstep[b][f] = ms;
+        s_okf[b][f] = ok;
       }
       __syncthreads();
       PF_MARK(0);
       pose_pass<CH, CACHED>(a, F, nchunks, p_try, s_ed, s_ef, s_wacc, parity ? s_part1 : s_part0, rank, csize);
       PF_MARK(1);
-      gather(s_new);
+      const double chi_f = gather(s_new);
       PF_MARK(2);
       // gain ratio and LM control (OptimizationAlgorithmLevenberg::solve), computed by every thread
       {
@@ -961,10 +991,10 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
         double temp = 0, scale = 0;
         mstep = 0;
         for (int f = 0; f < F; ++f) {
-          ok = ok && s_okf[f];
-          temp += s_new[f * PF_V + 27];
-          scale += s_fscale[f];
-          mstep = fmax(mstep, s_fstep[f]);
+          ok = ok && s_okf[b][f];
+          temp += __shfl_sync(0xffffffffu, chi_f, f);
+          scale += s_fscale[b][f];
+          mstep = fmax(mstep, s_fstep[b][f]);
         }
         if (!ok) temp = 1.7976931348623157e308;
         rho = (chi_cur - temp) * fast_rcp(scale + 1e-3);
@@ -984,7 +1014,6 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
           ni *= 2;
         }
       }
-      __syncthreads();                         // all threads have read s_fscale / s_okf before the next solve rewrites them
       ++qmax;
       ++trials;
       PF_MARK(3);
