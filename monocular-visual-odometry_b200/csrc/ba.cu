@@ -31,6 +31,9 @@
 #include <vector>
 #include "mvo_internal.h"
 #include "launch_pdl.cuh"
+#if !defined(__CUDACC__)
+#include "cuda_emu_mbarrier.h"     // CPU test tier (host compiler, tests/cpp on the include path): the emulated mbarrier
+#endif
 
 namespace cg = cooperative_groups;
 
@@ -38,7 +41,7 @@ namespace {
 
 constexpr int BA_T = 256;
 constexpr int BA_CLUSTER = 8;          // k_ba (Schur variant)
-constexpr int PF_MAXC = 16;            // k_ba_pose: up to 16 CTAs (non-portable cluster size)
+constexpr int PF_MAXC = 8;             // k_ba_pose: up to 8 CTAs (each receives the partials of all of them)
 constexpr int BA_MAXF = 16;
 constexpr int BA_NW = BA_T / 32;
 
@@ -561,11 +564,13 @@ size_t ba_smem_doubles(int F, int nact, int pc) {
 // edges are stored frame-major with their (fixed) 3-D point, every thread of the cluster takes
 // edges e = gtid, gtid + 4096, ...; the 27 sums per frame (21 Hessian + 6 gradient) and the robust
 // chi2 are reduced by a warp shuffle tree per frame segment, then across warps in shared memory,
-// then across the 8 CTAs through distributed shared memory (every CTA reads all partials in rank
-// order, so all CTAs hold identical state and decide identically).  The pass that evaluates a trial
-// step also linearises at the trial point, so an accepted step needs no second pass: one pass and
-// one cluster barrier per LM trial.  Per trial: solve (lane 0 of warp f for frame f) -> CTA barrier ->
-// pass -> CTA barrier -> cross-warp sum -> cluster barrier -> gather + decision (warp-local, no CTA barrier).
+// then across the 8 CTAs through distributed shared memory (every CTA pushes its partials into the
+// shared memory of all CTAs and sums what it received in rank order, so all CTAs hold identical state
+// and decide identically).  The pass that evaluates a trial step also linearises at the trial point, so
+// an accepted step needs no second pass: one pass and one exchange per LM trial, and no cluster barrier
+// between the first exchange and the exit.  Per trial: solve (lane 0 of warp f for frame f) -> CTA
+// barrier -> pass -> CTA barrier -> cross-warp sum and push -> wait for the CTA's mbarrier -> rank-order
+// sum + decision (warp-local, no CTA barrier).
 #ifndef MVO_PF_T
 #define MVO_PF_T 512
 #endif
@@ -711,7 +716,59 @@ __device__ __forceinline__ double warp_fold32(double (&v)[32], int lane) {
   return v[0];
 }
 
-// One pass over this CTA's chunks at poses `P` -> s_part[f*PF_V + q].  Thread (rank, tid) owns chunk
+// The push exchange of the pose LM: every CTA stores its partials straight into the receive area of each CTA of the cluster with
+// st.async, which counts the bytes on the receiver's mbarrier; a CTA has every partial of a round once that barrier's phase
+// completes.  The CPU test tier runs the same protocol on an emulated barrier (tests/cpp/cuda_emu_mbarrier.h).
+__device__ __forceinline__ void mbar_init(unsigned long long *bar, unsigned count) {
+#if defined(__CUDA_ARCH__)
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
+#elif !defined(__CUDACC__)
+  emu_mbar_init(bar, count);
+#endif
+}
+
+// makes initialised barriers visible to the st.async of the other CTAs (published by the next cluster barrier)
+__device__ __forceinline__ void mbar_init_fence() {
+#if defined(__CUDA_ARCH__)
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+#endif
+}
+
+// the barrier's one arrival per phase, with the bytes the phase has to receive
+__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long *bar, unsigned bytes) {
+#if defined(__CUDA_ARCH__)
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(bytes) : "memory");
+#elif !defined(__CUDACC__)
+  emu_mbar_arrive_expect_tx(bar, bytes);
+#endif
+}
+
+__device__ __forceinline__ void mbar_wait_parity(unsigned long long *bar, unsigned parity) {
+#if defined(__CUDA_ARCH__)
+  const unsigned b = (unsigned)__cvta_generic_to_shared(bar);
+  unsigned done;
+  do {
+    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+                 : "=r"(done) : "r"(b), "r"(parity) : "memory");
+  } while (!done);
+#elif !defined(__CUDACC__)
+  while (!emu_mbar_try_wait_parity(bar, parity)) {}
+#endif
+}
+
+// v -> CTA `rank`'s copy of *dst, 8 bytes counted on that CTA's copy of *bar (same shared-memory layout in every CTA)
+__device__ __forceinline__ void dsmem_push(double *dst, double v, unsigned long long *bar, unsigned rank) {
+#if defined(__CUDA_ARCH__)
+  unsigned rd, rb;
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rd) : "r"((unsigned)__cvta_generic_to_shared(dst)), "r"(rank));
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"((unsigned)__cvta_generic_to_shared(bar)), "r"(rank));
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.f64 [%0], %1, [%2];" ::"r"(rd), "d"(v), "r"(rb) : "memory");
+#elif !defined(__CUDACC__)
+  emu_st_async(dst, v, bar, rank);
+#endif
+}
+
+// One pass over this CTA's chunks at poses `P` -> row `rank` of every CTA's receive area, element f*PF_V + q.  Thread (rank, tid) owns chunk
 // rank*PF_T + tid: CH consecutive edges of ONE frame (host pads each frame's run to a multiple of CH with
 // frame -1), cached in shared memory (s_ed, SoA) when CACHED, so the LM trials never touch global memory.
 // Which chunk thread (rank, tid) of the cluster owns when the chunks are cached in shared memory: consecutive WARPS of chunks go to
@@ -724,7 +781,8 @@ __device__ __forceinline__ int pf_chunk_of(unsigned rank, int tid, unsigned csiz
 
 template <int CH, bool CACHED>
 __device__ void pose_pass(const PoseArgs &a, int F, int nchunks, const double *P, const double *s_ed, const int *s_ef,
-                          double *s_wacc /*[PF_NW][NV]*/, double *s_part, unsigned rank, unsigned csize) {
+                          double *s_wacc /*[PF_NW][NV]*/, double *recv /*this round's receive area [csize][NV]*/,
+                          unsigned long long *bar /*its barrier*/, unsigned rank, unsigned csize) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int NV = F * PF_V;
   // s_wacc is all-zero on entry (cleared at kernel start and re-cleared by the reduction below)
@@ -792,7 +850,7 @@ __device__ void pose_pass(const PoseArgs &a, int F, int nchunks, const double *P
     double s2 = 0;
 #pragma unroll
     for (int w = 0; w < PF_NW; ++w) s2 += part[w];
-    s_part[i] = s2;
+    for (unsigned r = 0; r < csize; ++r) dsmem_push(recv + rank * NV + i, s2, bar, r);      // this CTA's row of every receive area
   }
 }
 
@@ -801,11 +859,14 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), csize = cluster.num_blocks();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const long long t_start = clock64();       // cycles outside the trial loop, debug only (stats 4..7, 12, 13; s_c[3..6] on thread 0)
   pdl_wait();                                // PnP finish / the glue kernel wrote what this kernel reads (launch_pdl.cuh)
   pdl_launch_dependents();
+  const long long t_run = clock64();
   extern __shared__ __align__(16) double sm[];
+  __shared__ __align__(8) unsigned long long s_bar[2];     // one per receive area
   __shared__ int s_ef[PF_T];
-  __shared__ double s_c[8];                  // 0 lambda, 2 chi (initial)
+  __shared__ double s_c[8];                  // 0 lambda, 2 chi (initial), 3..6 cycle counts (debug)
   __shared__ double s_fscale[2][BA_MAXF], s_fstep[2][BA_MAXF];     // by trial parity: a solve never overwrites what a
   __shared__ int s_okf[2][BA_MAXF];                                // slower warp is still reading for the previous decision
   __shared__ int s_fslot[BA_MAXF], s_fcnt[BA_MAXF], s_cstart[BA_MAXF + 1], s_F;
@@ -835,7 +896,7 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
     if (rank == 0 && tid == 0) {
       a.st.out_info[0] = F;
       for (int f = 0; f < F; ++f) a.st.out_info[2 + f] = s_fslot[f];
-      a.st.out_info[1] = 0;                   // edges to map points that still exist, counted after the first cluster barrier
+      a.st.out_info[1] = 0;                   // edges to map points that still exist, counted after the cluster barrier below
     }
   }
   const int NV = F * PF_V;
@@ -843,11 +904,14 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
   double *s_try = s_pose + F * 12;           // F*12
   double *s_lin0 = s_try + F * 12;           // NV  linearisations (current / trial), ping-pong
   double *s_lin1 = s_lin0 + NV;              // NV
-  double *s_part0 = s_lin1 + NV;             // NV  partials, ping
-  double *s_part1 = s_part0 + NV;            // NV  partials, pong
-  double *s_dp = s_part1 + NV;               // F*6
-  double *s_wacc = s_dp + F * 6 + 2;         // PF_NW * NV
+  double *s_recv = s_lin1 + NV;              // [2][csize][NV]  partials of every CTA, by exchange parity
+  double *s_wacc = s_recv + 2 * csize * NV;  // PF_NW * NV
   double *s_ed = s_wacc + PF_NW * NV;        // CH*5*PF_T (CACHED only)
+  if (tid == 0) {
+    mbar_init(&s_bar[0], 1);
+    mbar_init(&s_bar[1], 1);
+    mbar_init_fence();
+  }
   if (STORE) { for (int i = tid; i < F * 12; i += PF_T) s_pose[i] = a.st.pose[(size_t)s_fslot[i / 12] * 12 + i % 12]; }
   else { for (int i = tid; i < F * 12; i += PF_T) s_pose[i] = a.poses[i]; }
   for (int i = tid; i < PF_NW * NV; i += PF_T) s_wacc[i] = 0;
@@ -889,25 +953,36 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
       ed[3 * PF_T] = real ? a.obs[2 * e] : -1e300; ed[4 * PF_T] = real ? a.obs[2 * e + 1] : 0;
     }
   }
-  __syncthreads();
-  int parity = 0;
-  // After the cluster barrier: sum the partials of all CTAs in rank order.  Warp w writes the rows of frames w, w + PF_NW, ..
-  // of dst, which only that warp's lane 0 reads (the solve of those frames), so no CTA barrier follows.  Every warp also sums
-  // the chi2 of each frame into lane f, the same sum as dst[f * PF_V + 27]: the LM decision is taken from registers.
+  // The one cluster barrier before the exchanges: every CTA's barriers are initialised before any CTA pushes into them.
+  cluster.sync();
+  const long long t_setup = clock64();
+  if (tid == 0) { s_c[3] = (double)(t_run - t_start); s_c[4] = (double)(t_setup - t_run); s_c[6] = (double)t_run; }
+  // Exchange x (0: the initial pass, then one per trial) lands in receive area x & 1 and completes phase x >> 1 of barrier
+  // x & 1.  Two areas suffice: a CTA pushes exchange x + 2 only after it has received every CTA's exchange x + 1, which each CTA
+  // sends after it has finished reading exchange x.  Bytes may land before the receiver arms the phase: the transaction count
+  // goes negative, and the phase cannot complete before the arrival that arms it.
+  int xchg = 0;
+  const unsigned xbytes = csize * (unsigned)NV * sizeof(double);
+  auto recv_of = [&](int x) { return s_recv + (x & 1) * csize * NV; };
+  // Sum the partials of all CTAs in rank order once they have landed.  Warp w writes the rows of frames w, w + PF_NW, .. of dst,
+  // which only that warp's lane 0 reads (the solve of those frames), so no CTA barrier follows.  Every warp also sums the chi2
+  // of each frame into lane f, the same sum as dst[f * PF_V + 27]: the LM decision is taken from registers.
   auto gather = [&](double *dst) -> double {
-    const double *mine = parity ? s_part1 : s_part0;
+    const double *in = recv_of(xchg);
+    unsigned long long *bar = &s_bar[xchg & 1];
+    if (tid == 0) mbar_arrive_expect_tx(bar, xbytes);
+    mbar_wait_parity(bar, (xchg >> 1) & 1);
     auto sum_ranks = [&](int i, int j, double &si, double &sj) {      // elements i and j (-1: none), all loads in flight together
       double v[PF_MAXC], u[PF_MAXC];
 #pragma unroll
       for (unsigned r = 0; r < PF_MAXC; ++r) {
-        v[r] = r < csize && i >= 0 ? *cluster.map_shared_rank(mine + i, r) : 0.0;
-        u[r] = r < csize && j >= 0 ? *cluster.map_shared_rank(mine + j, r) : 0.0;
+        v[r] = r < csize && i >= 0 ? in[r * NV + i] : 0.0;
+        u[r] = r < csize && j >= 0 ? in[r * NV + j] : 0.0;
       }
       si = 0; sj = 0;
 #pragma unroll
       for (unsigned r = 0; r < PF_MAXC; ++r) { si += v[r]; sj += u[r]; }       // fixed rank order: identical in every CTA
     };
-    cluster.sync();
     double chi_f, row, unused;
     if (warp < F) {                                                 // warp-uniform: the other warps issue only the chi2 loads
       sum_ranks(lane < F ? lane * PF_V + 27 : -1, lane < PF_V ? warp * PF_V + lane : -1, chi_f, row);
@@ -917,15 +992,15 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
     }
     for (int f = warp + PF_NW; f < F; f += PF_NW)                   // only when PF_NW < F
       if (lane < PF_V) { sum_ranks(f * PF_V + lane, -1, row, unused); dst[f * PF_V + lane] = row; }
-    parity ^= 1;
+    ++xchg;
     return chi_f;
   };
   double *s_cur = s_lin0, *s_new = s_lin1;
   double *p_cur = s_pose, *p_try = s_try;    // poses ping-pong like the linearisations
-  pose_pass<CH, CACHED>(a, F, nchunks, p_cur, s_ed, s_ef, s_wacc, parity ? s_part1 : s_part0, rank, csize);
+  pose_pass<CH, CACHED>(a, F, nchunks, p_cur, s_ed, s_ef, s_wacc, recv_of(xchg), &s_bar[xchg & 1], rank, csize);
   gather(s_cur);
   __syncthreads();                           // the initial chi2 and damping below read every frame's rows
-  if (STORE) {                               // behind the cluster barrier of the gather: out_info[1] has been zeroed
+  if (STORE) {                               // behind the cluster barrier above: out_info[1] has been zeroed
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) my_edges += __shfl_xor_sync(0xffffffffu, my_edges, o);
     if ((tid & 31) == 0 && my_edges) atomicAdd(&a.st.out_info[1], my_edges);
@@ -944,9 +1019,10 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
   }
   __syncthreads();
   const double chi_init = s_c[2];
-  int it = 0, trials = 0;
+  int it = 0, trials = 0, rejected = 0;
   bool terminate = false;
   long long ph[4] = {0, 0, 0, 0}, tmark = clock64();
+  if (tid == 0) s_c[5] = (double)(tmark - t_setup);
 #define PF_MARK(i) do { const long long t_ = clock64(); ph[i] += t_ - tmark; tmark = t_; } while (0)
   // LM control state lives in registers, replicated in every thread (all compute the same values)
   double lambda = s_c[0], ni = 2, chi_cur = s_c[2];
@@ -954,7 +1030,6 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
     int qmax = 0;
     double rho = 0;
     bool accepted = false, tiny = false;
-    double mstep = 0;
     do {
       // per-frame 6x6 solve + trial pose + this frame's share of the gain denominator (every CTA, identically), on lane 0 of
       // the warp that gathered the frame's rows
@@ -981,25 +1056,27 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
       }
       __syncthreads();
       PF_MARK(0);
-      pose_pass<CH, CACHED>(a, F, nchunks, p_try, s_ed, s_ef, s_wacc, parity ? s_part1 : s_part0, rank, csize);
+      pose_pass<CH, CACHED>(a, F, nchunks, p_try, s_ed, s_ef, s_wacc, recv_of(xchg), &s_bar[xchg & 1], rank, csize);
       PF_MARK(1);
+      // gain ratio and LM control (OptimizationAlgorithmLevenberg::solve), computed by every thread.  Status, gain denominator and
+      // step size of the frames depend on the solve alone: reduced while the partials of the other CTAs are in flight.
+      bool ok = true;
+      double scale = 0, mstep = 0;
+      for (int f = 0; f < F; ++f) {
+        ok = ok && s_okf[b][f];
+        scale += s_fscale[b][f];
+        mstep = fmax(mstep, s_fstep[b][f]);
+      }
+      const double rscale = fast_rcp(scale + 1e-3);
+      tiny = a.step_tol > 0 && ok && mstep < a.step_tol;
       const double chi_f = gather(s_new);
       PF_MARK(2);
-      // gain ratio and LM control (OptimizationAlgorithmLevenberg::solve), computed by every thread
       {
-        bool ok = true;
-        double temp = 0, scale = 0;
-        mstep = 0;
-        for (int f = 0; f < F; ++f) {
-          ok = ok && s_okf[b][f];
-          temp += __shfl_sync(0xffffffffu, chi_f, f);
-          scale += s_fscale[b][f];
-          mstep = fmax(mstep, s_fstep[b][f]);
-        }
+        double temp = 0;
+        for (int f = 0; f < F; ++f) temp += __shfl_sync(0xffffffffu, chi_f, f);
         if (!ok) temp = 1.7976931348623157e308;
-        rho = (chi_cur - temp) * fast_rcp(scale + 1e-3);
+        rho = (chi_cur - temp) * rscale;
         accepted = rho > 0 && isfinite(temp);
-        tiny = a.step_tol > 0 && ok && mstep < a.step_tol;
         if (accepted) {
           const double tr = 2 * rho - 1;
           double alpha = 1. - tr * tr * tr;
@@ -1012,6 +1089,7 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
         } else {
           lambda *= ni;
           ni *= 2;
+          ++rejected;
         }
       }
       ++qmax;
@@ -1025,17 +1103,31 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
     // step is not applied, exactly as g2o would restore it.
     if (tiny) terminate = true;
   }
-  cluster.sync();       // nobody leaves while a neighbour may still read its partials
+  const long long t_loop = clock64();
+  cluster.sync();       // the last pushes of a CTA may still be landing in a peer: nobody leaves before every CTA has them
+  const long long t_end = clock64();
   if (rank == 0) {
     if (STORE) { for (int i = tid; i < F * 12; i += PF_T) a.st.pose[(size_t)s_fslot[i / 12] * 12 + i % 12] = p_cur[i]; }
     else { for (int i = tid; i < F * 12; i += PF_T) a.poses[i] = p_cur[i]; }
-    if (tid == 0) { a.stats[0] = chi_init; a.stats[1] = chi_cur; a.stats[2] = it; a.stats[3] = lambda; a.stats[15] = trials; for (int q = 0; q < 4; ++q) a.stats[8 + q] = (double)ph[q]; }
+    if (tid == 0) {
+      a.stats[0] = chi_init; a.stats[1] = chi_cur; a.stats[2] = it; a.stats[3] = lambda; a.stats[15] = trials;
+      for (int q = 0; q < 4; ++q) a.stats[8 + q] = (double)ph[q];
+      a.stats[4] = s_c[4];                         // edge gather into shared memory and the start barrier
+      a.stats[5] = s_c[5];                         // initial pass, exchange and damping
+      a.stats[6] = (double)(t_end - t_loop);       // exit barrier
+      a.stats[7] = rejected;
+      a.stats[12] = s_c[3];                        // wait for the predecessor (programmatic dependent launch)
+      a.stats[13] = (double)t_end - s_c[6];        // the whole kernel after that wait
+    }
   }
 }
 
-size_t pose_smem_doubles(int F, int cached_ch) {
-  return (size_t)F * 24 + 4 * (size_t)F * PF_V + (size_t)F * 6 + 2 + (size_t)PF_NW * F * PF_V + (size_t)cached_ch * 5 * PF_T + 8;
+constexpr size_t pose_smem_doubles(int F, int cached_ch, int csize) {
+  return (size_t)F * 24 + 2 * (size_t)F * PF_V + 2 * (size_t)csize * F * PF_V + (size_t)PF_NW * F * PF_V + (size_t)cached_ch * 5 * PF_T;
 }
+// The H100 lets a block opt in to 227 KB of shared memory; k_ba_pose's static __shared__ arrays take less than 3 KB of it.
+constexpr size_t PF_SMEM_MAX = 224 * 1024;
+static_assert(pose_smem_doubles(BA_MAXF, 4, PF_MAXC) * sizeof(double) <= PF_SMEM_MAX, "largest pose LM does not fit shared memory");
 
 }  // namespace
 
@@ -1045,9 +1137,8 @@ static int pose_cluster_size() {
 }
 
 static int pose_launch(mvo_ctx *ctx, void (*kern)(PoseArgs), const PoseArgs &a, int csz, size_t smem) {
-  if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "pose BA: shared memory %zu B", smem);
+  if (smem > PF_SMEM_MAX) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "pose BA: shared memory %zu B", smem);
   MVO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  if (csz > 8) MVO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   {
     KTimer kt(ctx, KC_BA);
     MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)csz, PF_T, smem, (unsigned)csz, kern, a));      // one cluster; may start under its predecessor's tail
@@ -1071,7 +1162,7 @@ int mvo_ba_pose_launch(mvo_ctx *ctx, int F, int E, int chunk, const int32_t *d_e
   static const int env_refit = getenv("MVO_REFIT_CLUSTER") ? atoi(getenv("MVO_REFIT_CLUSTER")) : 0;      // A/B hook for the one-frame problems
   const int csz = (env_refit >= 1 && env_refit <= PF_MAXC) ? env_refit : pose_cluster_size();
   const bool cached = chunk >= 1 && chunk <= 4 && E / chunk <= csz * PF_T;
-  const size_t smem = pose_smem_doubles(F, cached ? chunk : 0) * sizeof(double);
+  const size_t smem = pose_smem_doubles(F, cached ? chunk : 0, csz) * sizeof(double);
   void (*kern)(PoseArgs) = k_ba_pose<1, false, false>;
   if (cached) {
     switch (chunk) {
@@ -1103,7 +1194,7 @@ int mvo_ba_pose_store_launch(mvo_ctx *ctx, const MvoPoseStore &st, int e_upper, 
   a.huber = huber; a.step_tol = step_tol;
   a.stats = d_stats;
   a.st = st;
-  const size_t smem = pose_smem_doubles(st.nslots, chunk) * sizeof(double);
+  const size_t smem = pose_smem_doubles(st.nslots, chunk, csz) * sizeof(double);
   void (*kern)(PoseArgs) = nullptr;
   switch (chunk) {
     case 1: kern = k_ba_pose<1, true, true>; break;
@@ -1200,7 +1291,10 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
       T[15] = 1;
     }
     if (stats) memcpy(stats, h_stats, 32);
-    if (getenv("MVO_BA_DEBUG")) fprintf(stderr, "k_ba_pose: F=%d E=%d it=%.0f trials=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f\n", F, E, h_stats[2], h_stats[15], h_stats[8], h_stats[9], h_stats[10], h_stats[11]);
+    if (getenv("MVO_BA_DEBUG"))
+      fprintf(stderr, "k_ba_pose: F=%d E=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f | "
+              "pdl_wait=%.0f setup=%.0f init=%.0f exit=%.0f kernel=%.0f\n", F, E, h_stats[2], h_stats[15], h_stats[7], h_stats[8], h_stats[9],
+              h_stats[10], h_stats[11], h_stats[12], h_stats[4], h_stats[5], h_stats[6], h_stats[13]);
     return MVO_OK;
   }
 

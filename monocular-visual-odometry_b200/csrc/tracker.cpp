@@ -1259,8 +1259,9 @@ static int track_device(mvo_tracker *t, ExtractJob &job, int slot, double *T_w_c
     r.ba_edges = h_info[1];
     static const bool ba_dbg = getenv("MVO_BA_DEBUG") != nullptr;
     if (ba_dbg)
-      fprintf(stderr, "k_ba_pose(store): F=%d E=%d it=%.0f trials=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f\n", F, h_info[1],
-              h_stats[2], h_stats[15], h_stats[8], h_stats[9], h_stats[10], h_stats[11]);
+      fprintf(stderr, "k_ba_pose(store): F=%d E=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f | "
+              "pdl_wait=%.0f setup=%.0f init=%.0f exit=%.0f kernel=%.0f\n", F, h_info[1], h_stats[2], h_stats[15], h_stats[7], h_stats[8],
+              h_stats[9], h_stats[10], h_stats[11], h_stats[12], h_stats[4], h_stats[5], h_stats[6], h_stats[13]);
   }
   TMARK(2);
   if (dbg && ++nacc % 50 == 0) {
