@@ -46,7 +46,7 @@ constexpr int BA_MAXF = 16;
 constexpr int BA_NW = BA_T / 32;
 
 struct BaArgs {
-  int F, P, E, iters, fix_points, fix_first, use_huber, pc;
+  int F, P, E, iters, fix_first, use_huber, pc;
   double f, cx, cy, i00, i01, i10, i11, huber;
   const int32_t *pt_start;
   const int32_t *e_frame;
@@ -171,7 +171,6 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
   // this CTA's points
   const int per = (a.P + (int)csize - 1) / (int)csize;
   const int p0 = min((int)rank * per, a.P), p1 = min(p0 + per, a.P);
-  const bool freep = !a.fix_points;
   double chi_init = 0;
   int it = 0;
   bool terminate = false;
@@ -227,17 +226,9 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
           double OA[6];
 #pragma unroll
           for (int c = 0; c < 3; ++c) { OA[c] = o00 * A[c] + o01 * A[3 + c]; OA[3 + c] = o10 * A[c] + o11 * A[3 + c]; }
-          if (freep) {
-            blv[0] += A[0] * r0 + A[3] * r1; blv[1] += A[1] * r0 + A[4] * r1; blv[2] += A[2] * r0 + A[5] * r1;
-            hl[0] += A[0] * OA[0] + A[3] * OA[3]; hl[1] += A[0] * OA[1] + A[3] * OA[4]; hl[2] += A[0] * OA[2] + A[3] * OA[5];
-            hl[3] += A[1] * OA[1] + A[4] * OA[4]; hl[4] += A[1] * OA[2] + A[4] * OA[5]; hl[5] += A[2] * OA[2] + A[5] * OA[5];
-            if (pose_act) {
-#pragma unroll
-              for (int r = 0; r < 6; ++r)
-#pragma unroll
-                for (int c = 0; c < 3; ++c) wlf[r * 3 + c] += B[r] * OA[c] + B[6 + r] * OA[3 + c];
-            }
-          }
+          blv[0] += A[0] * r0 + A[3] * r1; blv[1] += A[1] * r0 + A[4] * r1; blv[2] += A[2] * r0 + A[5] * r1;
+          hl[0] += A[0] * OA[0] + A[3] * OA[3]; hl[1] += A[0] * OA[1] + A[3] * OA[4]; hl[2] += A[0] * OA[2] + A[3] * OA[5];
+          hl[3] += A[1] * OA[1] + A[4] * OA[4]; hl[4] += A[1] * OA[2] + A[4] * OA[5]; hl[5] += A[2] * OA[2] + A[5] * OA[5];
           if (pose_act) {
             double OB[12];
 #pragma unroll
@@ -250,9 +241,17 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
 #pragma unroll
             for (int r = 0; r < 6; ++r) hp[21 + r] += B[r] * r0 + B[6 + r] * r1;
           }
+          // W = B^T Omega A in a block of its own, after the Hpp terms: merged into the block above, or ahead of it, the
+          // linearisation spills at the 255-register limit
+          if (pose_act) {
+#pragma unroll
+            for (int r = 0; r < 6; ++r)
+#pragma unroll
+              for (int c = 0; c < 3; ++c) wlf[r * 3 + c] += B[r] * OA[c] + B[6 + r] * OA[3 + c];
+          }
           ++k;
         }
-        if (freep && act && pose_act) {
+        if (act && pose_act) {
           double *wd = a.Wd + ((size_t)l * F + f) * 18;
 #pragma unroll
           for (int q = 0; q < 18; ++q) wd[q] = wlf[q];
@@ -265,7 +264,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
           }
         }
       }
-      if (freep && act) {
+      if (act) {
 #pragma unroll
         for (int q = 0; q < 6; ++q) a.Hll[(size_t)l * 6 + q] = hl[q];
         a.bl[3 * l] = blv[0]; a.bl[3 * l + 1] = blv[1]; a.bl[3 * l + 2] = blv[2];
@@ -303,7 +302,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
       s_ctl[2] = s_full[F * 27];
       if (it == 0) {
         // computeLambdaInit: tau * max |diag| over all non-fixed vertices, tau = 1e-5
-        double md = freep ? s_full[F * 27 + 1] : 0;
+        double md = s_full[F * 27 + 1];
         for (int f = 0; f < F; ++f)
           if (s_pidx[f] >= 0) {
             const double *h = s_full + f * 27;
@@ -322,63 +321,61 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
     double rho = 0;
     do {
       const double lambda = s_ctl[0];
-      // ---- phase C: Schur partials (free points only) ----
+      // ---- phase C: Schur partials ----
       for (int i = tid; i < NC; i += BA_T) s_partC[i] = 0;
       bool inv_ok = true;
-      if (freep) {
-        double *s_Y = s_u;                                   // [pc][F][18]
-        double *s_W = s_Y + (size_t)a.pc * F * 18;           // [pc][F][18]
-        double *s_b = s_W + (size_t)a.pc * F * 18;           // [pc][3]
-        for (int c0 = p0; c0 < p1; c0 += a.pc) {
-          const int cn = min(a.pc, p1 - c0);
-          __syncthreads();
-          for (int i = tid; i < cn * F; i += BA_T) {
-            const int li = i / F, f = i - li * F, l = c0 + li;
-            double *Ys = s_Y + (size_t)i * 18, *Ws = s_W + (size_t)i * 18;
-            const bool has = a.pt_start[l + 1] > a.pt_start[l];
-            double hi[6] = {0, 0, 0, 0, 0, 0};
-            if (has) { if (!inv3_sym(a.Hll + (size_t)l * 6, lambda, hi)) { inv_ok = false; } }
-            if (f == 0) {
+      double *s_Y = s_u;                                   // [pc][F][18]
+      double *s_W = s_Y + (size_t)a.pc * F * 18;           // [pc][F][18]
+      double *s_b = s_W + (size_t)a.pc * F * 18;           // [pc][3]
+      for (int c0 = p0; c0 < p1; c0 += a.pc) {
+        const int cn = min(a.pc, p1 - c0);
+        __syncthreads();
+        for (int i = tid; i < cn * F; i += BA_T) {
+          const int li = i / F, f = i - li * F, l = c0 + li;
+          double *Ys = s_Y + (size_t)i * 18, *Ws = s_W + (size_t)i * 18;
+          const bool has = a.pt_start[l + 1] > a.pt_start[l];
+          double hi[6] = {0, 0, 0, 0, 0, 0};
+          if (has) { if (!inv3_sym(a.Hll + (size_t)l * 6, lambda, hi)) { inv_ok = false; } }
+          if (f == 0) {
 #pragma unroll
-              for (int q = 0; q < 6; ++q) a.Hinv[(size_t)l * 6 + q] = hi[q];
-              s_b[li * 3] = a.bl[3 * l]; s_b[li * 3 + 1] = a.bl[3 * l + 1]; s_b[li * 3 + 2] = a.bl[3 * l + 2];
+            for (int q = 0; q < 6; ++q) a.Hinv[(size_t)l * 6 + q] = hi[q];
+            s_b[li * 3] = a.bl[3 * l]; s_b[li * 3 + 1] = a.bl[3 * l + 1]; s_b[li * 3 + 2] = a.bl[3 * l + 2];
+          }
+          if (has && s_pidx[f] >= 0) {
+            const double *wd = a.Wd + ((size_t)l * F + f) * 18;
+#pragma unroll
+            for (int r = 0; r < 6; ++r) {
+              const double w0 = wd[r * 3], w1 = wd[r * 3 + 1], w2 = wd[r * 3 + 2];
+              Ws[r * 3] = w0; Ws[r * 3 + 1] = w1; Ws[r * 3 + 2] = w2;
+              Ys[r * 3] = w0 * hi[0] + w1 * hi[1] + w2 * hi[2];
+              Ys[r * 3 + 1] = w0 * hi[1] + w1 * hi[3] + w2 * hi[4];
+              Ys[r * 3 + 2] = w0 * hi[2] + w1 * hi[4] + w2 * hi[5];
             }
-            if (has && s_pidx[f] >= 0) {
-              const double *wd = a.Wd + ((size_t)l * F + f) * 18;
+          } else {
 #pragma unroll
-              for (int r = 0; r < 6; ++r) {
-                const double w0 = wd[r * 3], w1 = wd[r * 3 + 1], w2 = wd[r * 3 + 2];
-                Ws[r * 3] = w0; Ws[r * 3 + 1] = w1; Ws[r * 3 + 2] = w2;
-                Ys[r * 3] = w0 * hi[0] + w1 * hi[1] + w2 * hi[2];
-                Ys[r * 3 + 1] = w0 * hi[1] + w1 * hi[3] + w2 * hi[4];
-                Ys[r * 3 + 2] = w0 * hi[2] + w1 * hi[4] + w2 * hi[5];
-              }
-            } else {
-#pragma unroll
-              for (int q = 0; q < 18; ++q) { Ws[q] = 0; Ys[q] = 0; }
+            for (int q = 0; q < 18; ++q) { Ws[q] = 0; Ys[q] = 0; }
+          }
+        }
+        __syncthreads();
+        for (int o = tid; o < NC; o += BA_T) {
+          double acc = 0;
+          if (o < n * n) {
+            const int i = o / n, j = o - i * n;
+            const int fa = s_act[i / 6], ra = i % 6, fb = s_act[j / 6], rb = j % 6;
+            const double *yp = s_Y + ((size_t)fa * 18 + ra * 3), *wp = s_W + ((size_t)fb * 18 + rb * 3);
+            for (int li = 0; li < cn; ++li) {
+              const double *y = yp + (size_t)li * F * 18, *w = wp + (size_t)li * F * 18;
+              acc += y[0] * w[0] + y[1] * w[1] + y[2] * w[2];
+            }
+          } else {
+            const int i = o - n * n, fa = s_act[i / 6], ra = i % 6;
+            const double *yp = s_Y + ((size_t)fa * 18 + ra * 3);
+            for (int li = 0; li < cn; ++li) {
+              const double *y = yp + (size_t)li * F * 18, *b = s_b + li * 3;
+              acc += y[0] * b[0] + y[1] * b[1] + y[2] * b[2];
             }
           }
-          __syncthreads();
-          for (int o = tid; o < NC; o += BA_T) {
-            double acc = 0;
-            if (o < n * n) {
-              const int i = o / n, j = o - i * n;
-              const int fa = s_act[i / 6], ra = i % 6, fb = s_act[j / 6], rb = j % 6;
-              const double *yp = s_Y + ((size_t)fa * 18 + ra * 3), *wp = s_W + ((size_t)fb * 18 + rb * 3);
-              for (int li = 0; li < cn; ++li) {
-                const double *y = yp + (size_t)li * F * 18, *w = wp + (size_t)li * F * 18;
-                acc += y[0] * w[0] + y[1] * w[1] + y[2] * w[2];
-              }
-            } else {
-              const int i = o - n * n, fa = s_act[i / 6], ra = i % 6;
-              const double *yp = s_Y + ((size_t)fa * 18 + ra * 3);
-              for (int li = 0; li < cn; ++li) {
-                const double *y = yp + (size_t)li * F * 18, *b = s_b + li * 3;
-                acc += y[0] * b[0] + y[1] * b[1] + y[2] * b[2];
-              }
-            }
-            s_partC[o] += acc;
-          }
+          s_partC[o] += acc;
         }
       }
       if (tid == 0) s_partE[2] = 1.0;
@@ -390,7 +387,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
       // ---- phase D: assemble and solve the pose system (every CTA, identically) ----
       for (int o = tid; o < NC; o += BA_T) {
         double s = 0;
-        if (freep) for (unsigned r = 0; r < csize; ++r) s += *cluster.map_shared_rank(s_partC + o, r);
+        for (unsigned r = 0; r < csize; ++r) s += *cluster.map_shared_rank(s_partC + o, r);
         if (o < n * n) {
           const int i = o / n, j = o - i * n;
           double h = 0;
@@ -453,7 +450,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
       for (int l = p0 + tid; l < p1; l += BA_T) {
         double X[3] = {pts[3 * l], pts[3 * l + 1], pts[3 * l + 2]};
         const int kb = a.pt_start[l], ke = a.pt_start[l + 1];
-        if (freep && ok && ke > kb) {
+        if (ok && ke > kb) {
           double c[3] = {a.bl[3 * l], a.bl[3 * l + 1], a.bl[3 * l + 2]};
           const double b0 = c[0], b1 = c[1], b2 = c[2];
           for (int f = 0; f < F; ++f) {
@@ -470,7 +467,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
           X[0] += d0; X[1] += d1; X[2] += d2;
           scale_t += d0 * (lambda * d0 + b0) + d1 * (lambda * d1 + b1) + d2 * (lambda * d2 + b2);
         }
-        if (freep) { pts_try[3 * l] = X[0]; pts_try[3 * l + 1] = X[1]; pts_try[3 * l + 2] = X[2]; }
+        pts_try[3 * l] = X[0]; pts_try[3 * l + 1] = X[1]; pts_try[3 * l + 2] = X[2];
         for (int k = kb; k < ke; ++k) {
           double x, y, z, e0, e1;
           edge_residual(s_try + 12 * a.e_frame[k], X, a.obs[2 * k], a.obs[2 * k + 1], a, x, y, z, e0, e1);
@@ -523,10 +520,8 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
       rho = s_ctl[3];
       if (s_ctl[4] != 0) {              // accepted: trial state becomes current
         for (int i = tid; i < F * 12; i += BA_T) s_pose[i] = s_try[i];
-        if (freep) {
-          __syncthreads();
-          if (tid == 0) s_ctl[6] = (s_ctl[6] != 0) ? 0.0 : 1.0;
-        }
+        __syncthreads();
+        if (tid == 0) s_ctl[6] = (s_ctl[6] != 0) ? 0.0 : 1.0;
       }
       __syncthreads();
       ++qmax;
@@ -1159,8 +1154,7 @@ int mvo_ba_pose_launch(mvo_ctx *ctx, int F, int E, int chunk, const int32_t *d_e
   a.i00 = info[0]; a.i01 = info[1]; a.i10 = info[2]; a.i11 = info[3];
   a.huber = huber; a.step_tol = step_tol;
   a.e_frame = d_eframe; a.X = d_X; a.obs = d_obs; a.poses = d_poses; a.stats = d_stats;
-  static const int env_refit = getenv("MVO_REFIT_CLUSTER") ? atoi(getenv("MVO_REFIT_CLUSTER")) : 0;      // A/B hook for the one-frame problems
-  const int csz = (env_refit >= 1 && env_refit <= PF_MAXC) ? env_refit : pose_cluster_size();
+  const int csz = pose_cluster_size();
   const bool cached = chunk >= 1 && chunk <= 4 && E / chunk <= csz * PF_T;
   const size_t smem = pose_smem_doubles(F, cached ? chunk : 0, csz) * sizeof(double);
   void (*kern)(PoseArgs) = k_ba_pose<1, false, false>;
@@ -1203,6 +1197,24 @@ int mvo_ba_pose_store_launch(mvo_ctx *ctx, const MvoPoseStore &st, int e_upper, 
     default: kern = k_ba_pose<4, true, true>; break;
   }
   return pose_launch(ctx, kern, a, csz, smem);
+}
+
+// g2o_ba.cpp:183-190: camera->world T_w_c (4x4 row-major) -> world->camera [R|t] = (T_w_c)^-1 (R row-major, then t)
+static void T_w_c_to_Rt(const double *T, double *q) {
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) q[i * 3 + j] = T[j * 4 + i];
+    q[9 + i] = -(T[0 * 4 + i] * T[3] + T[1 * 4 + i] * T[7] + T[2 * 4 + i] * T[11]);
+  }
+}
+
+// g2o_ba.cpp:298-305: world->camera [R|t] -> camera->world T_w_c
+static void Rt_to_T_w_c(const double *p, double *T) {
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) T[i * 4 + j] = p[j * 3 + i];
+    T[i * 4 + 3] = -(p[i] * p[9] + p[3 + i] * p[10] + p[6 + i] * p[11]);
+  }
+  T[12] = T[13] = T[14] = 0;
+  T[15] = 1;
 }
 
 // Shared driver for bundleAdjustment and optimizeSingleFrame.
@@ -1264,14 +1276,7 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
         for (; w % chunk; ++w) { hf[w] = -1; hX[3 * w] = hX[3 * w + 1] = 0; hX[3 * w + 2] = 1; hobs[2 * w] = hobs[2 * w + 1] = 0; }
       }
     }
-    for (int f = 0; f < F; ++f) {                                 // g2o_ba.cpp:183-190: world->camera = (T_w_c)^-1
-      const double *T = poses_T_w_c + 16 * f;
-      double *q = hpose + 12 * f;
-      for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j) q[i * 3 + j] = T[j * 4 + i];
-        q[9 + i] = -(T[0 * 4 + i] * T[3] + T[1 * 4 + i] * T[7] + T[2 * 4 + i] * T[11]);
-      }
-    }
+    for (int f = 0; f < F; ++f) T_w_c_to_Rt(poses_T_w_c + 16 * f, hpose + 12 * f);
     MVO_CUDA(ctx, cudaMemcpyAsync(d, h, in_end, cudaMemcpyHostToDevice, ctx->stream));
     MVO_TRY(mvo_ba_pose_launch(ctx, F, Ep, chunk, (const int32_t *)(d + o_fr), (const double *)(d + o_X), (const double *)(d + o_obs),
                                K[0], K[0], K[2], K[5], info, iterations, use_huber && ctx->prm.ba_huber_delta > 0,
@@ -1280,16 +1285,7 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
     MVO_CUDA(ctx, cudaMemcpyAsync(hpose, d + o_pose, (size_t)F * 96, cudaMemcpyDeviceToHost, ctx->stream));
     MVO_CUDA(ctx, cudaMemcpyAsync(h_stats, d + o_stats, 128, cudaMemcpyDeviceToHost, ctx->stream));
     MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (int f = 0; f < F; ++f) {                                 // g2o_ba.cpp:298-305
-      const double *p = hpose + 12 * f;
-      double *T = poses_T_w_c + 16 * f;
-      for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j) T[i * 4 + j] = p[j * 3 + i];
-        T[i * 4 + 3] = -(p[i] * p[9] + p[3 + i] * p[10] + p[6 + i] * p[11]);
-      }
-      T[12] = T[13] = T[14] = 0;
-      T[15] = 1;
-    }
+    for (int f = 0; f < F; ++f) Rt_to_T_w_c(hpose + 12 * f, poses_T_w_c + 16 * f);
     if (stats) memcpy(stats, h_stats, 32);
     if (getenv("MVO_BA_DEBUG"))
       fprintf(stderr, "k_ba_pose: F=%d E=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f | "
@@ -1316,16 +1312,8 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
       e_obs[2 * i + 1] = obs[2 * order[i] + 1];
     }
   }
-  // g2o_ba.cpp:183-190: world->camera = (T_w_c)^-1
   std::vector<double> pose12((size_t)F * 12), pts_d(3 * (size_t)std::max(P, 1));
-  for (int f = 0; f < F; ++f) {
-    const double *T = poses_T_w_c + 16 * f;
-    double *o = pose12.data() + 12 * f;
-    for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j) o[i * 3 + j] = T[j * 4 + i];
-      o[9 + i] = -(T[0 * 4 + i] * T[3] + T[1 * 4 + i] * T[7] + T[2 * 4 + i] * T[11]);
-    }
-  }
+  for (int f = 0; f < F; ++f) T_w_c_to_Rt(poses_T_w_c + 16 * f, pose12.data() + 12 * f);
   for (int i = 0; i < 3 * P; ++i) pts_d[i] = points[i];
 
   auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
@@ -1340,7 +1328,7 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
   const size_t o_hll = o;   o = al(o + (size_t)P * 48 + 48);
   const size_t o_bl = o;    o = al(o + (size_t)P * 24 + 24);
   const size_t o_hinv = o;  o = al(o + (size_t)P * 48 + 48);
-  const size_t o_wd = o;    o = al(o + (fix_points ? 8 : (size_t)P * F * 144 + 144));
+  const size_t o_wd = o;    o = al(o + (size_t)P * F * 144 + 144);
   const size_t o_stats = o; o = al(o + 256);
   MVO_TRY(mvo_reserve(ctx, ctx->ba_buf, o));
   MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_a, in_end + 4096));
@@ -1353,7 +1341,7 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
   MVO_CUDA(ctx, cudaMemcpyAsync(d, h, in_end, cudaMemcpyHostToDevice, ctx->stream));
 
   BaArgs a;
-  a.F = F; a.P = P; a.E = E; a.iters = iterations; a.fix_points = fix_points ? 1 : 0; a.fix_first = fix_first;
+  a.F = F; a.P = P; a.E = E; a.iters = iterations; a.fix_first = fix_first;
   a.use_huber = use_huber && ctx->prm.ba_huber_delta > 0;
   a.f = K[0]; a.cx = K[2]; a.cy = K[5];                      // g2o_ba.cpp:219-220: fy is ignored
   a.i00 = info[0]; a.i01 = info[1]; a.i10 = info[2]; a.i11 = info[3];
@@ -1391,23 +1379,14 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
   MVO_CUDA(ctx, cudaMemcpyAsync(h_pose, a.poses, (size_t)F * 96, cudaMemcpyDeviceToHost, ctx->stream));
   MVO_CUDA(ctx, cudaMemcpyAsync(h_stats, a.stats, 128, cudaMemcpyDeviceToHost, ctx->stream));
   MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (!fix_points && update_points && P > 0) {
+  if (update_points && P > 0) {
     const int sel = *(int32_t *)((uint8_t *)h_stats + 32);
     MVO_CUDA(ctx, cudaMemcpyAsync(h + o_pa, sel ? a.pts_b : a.pts_a, (size_t)P * 24, cudaMemcpyDeviceToHost, ctx->stream));
     MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     const double *pd = (const double *)(h + o_pa);
     for (int i = 0; i < 3 * P; ++i) points[i] = (float)pd[i];      // g2o_ba.cpp:313-315
   }
-  for (int f = 0; f < F; ++f) {                                     // g2o_ba.cpp:298-305: back to camera->world
-    const double *p = h_pose + 12 * f;
-    double *T = poses_T_w_c + 16 * f;
-    for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j) T[i * 4 + j] = p[j * 3 + i];
-      T[i * 4 + 3] = -(p[i] * p[9] + p[3 + i] * p[10] + p[6 + i] * p[11]);
-    }
-    T[12] = T[13] = T[14] = 0;
-    T[15] = 1;
-  }
+  for (int f = 0; f < F; ++f) Rt_to_T_w_c(h_pose + 12 * f, poses_T_w_c + 16 * f);
   if (stats) memcpy(stats, h_stats, 32);
   if (getenv("MVO_BA_DEBUG")) {
     fprintf(stderr, "k_ba: F=%d P=%d E=%d it=%.0f trials=%.0f cycles A=%.0f B=%.0f C=%.0f D=%.0f E=%.0f F=%.0f sync=%.0f\n", F, P, E,

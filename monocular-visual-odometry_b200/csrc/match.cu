@@ -17,7 +17,6 @@
 //
 // Arithmetic per pair, Hamming: 8 LOP3 (xor) + 8 LOP3 (carry-save adders) + 4 POPC + 3 adds
 // + 1 pack + 1 min.  No tensor cores: integer/POPC-issue bound (SURVEY.md §8d).
-#include <stdlib.h>
 #include "mvo_internal.h"
 #include "launch_pdl.cuh"
 
@@ -195,8 +194,9 @@ int mvo_match_launch_ndev(mvo_ctx *ctx, int mode, const uint8_t *d_d1, const flo
     return MVO_OK;
   }
   const int qtiles = (n1 + kQ - 1) / kQ;
-  // enough CTAs for ~2 waves over the SMs, chunks of at least 32 and at most kMaxChunk trains
-  static const int waves = getenv("MVO_MATCH_WAVES") ? atoi(getenv("MVO_MATCH_WAVES")) : 4;      // CTAs per SM-count: on the H100, 2 and 4 are within run-to-run noise of the VO pass, 8 is slower
+  // about 4 CTAs per SM (on the H100, 2 and 4 are within run-to-run noise of the VO pass, 8 is slower), chunks of at least 32
+  // and at most kMaxChunk trains
+  const int waves = 4;
   int nsplit = (waves * ctx->sm_count + qtiles - 1) / qtiles;
   const int min_split = (n2 + kMaxChunk - 1) / kMaxChunk;
   const int max_split = (n2 + 31) / 32;

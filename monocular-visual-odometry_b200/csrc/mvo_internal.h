@@ -208,7 +208,6 @@ int mvo_trk_set_map_ids(mvo_tracker *t, const float *pts3d, const uint8_t *desc,
 int mvo_trk_push_frame(mvo_tracker *t, const double *T_w_c, const int32_t *ids, const int32_t *kp_idx, const float *obs_xy, int n);
 int mvo_trk_append_links(mvo_tracker *t, int k, const int32_t *ids, const int32_t *kp_idx, const float *obs_xy, int n);
 int mvo_trk_links(mvo_tracker *t, int k, int32_t *ids, int32_t *kp_idx, int cap, int *n);
-int mvo_trk_counters(mvo_tracker *t, int32_t *visible, int32_t *matched, int n);
 // keyframe insertion in one submission / one synchronisation (tracker.cpp); the pointers address the context's pinned staging
 // buffer and stay valid until the next fetch
 struct MvoKfFetch {

@@ -14,7 +14,7 @@
 //                 reject, cornerScore<16> only for survivors, 3x3 NMS, raster-ordered emit
 //   k_select      one CTA per frame: candidate compaction + first-come grid selection, restated
 //                 as rank-in-cell < max_per_cell and an ordered prefix count (deterministic)
-//   k_blur        7x7 sigma-2 Gaussian, float separable, round-half-even (ORB's descriptor blur)
+//   k_blur2       7x7 sigma-2 Gaussian, float separable, round-half-even (ORB's descriptor blur; orb_variants.cuh)
 //   k_describe    one warp per keypoint: Harris response, intensity-centroid angle, 256 steered
 //                 BRIEF tests (lane i produces descriptor byte i)
 // Float formulas that OpenCV evaluates without FMA use __fmul_rn/__fadd_rn explicitly.
@@ -1024,58 +1024,7 @@ constexpr int BLUR_TW = 128, BLUR_TH = 16;
 // all pyramid levels of a frame in ONE launch: blockIdx.x walks the tiles of level 0, then level 1, ...
 struct BlurTiles { int first[MVO_MAX_LEVELS + 1]; int nx[MVO_MAX_LEVELS]; };
 
-__global__ void __launch_bounds__(256)
-k_blur(OrbPlanDev plan, BlurTiles tiles, uint8_t *__restrict__ planes) {
-  pdl_wait();
-  pdl_launch_dependents();
-  __shared__ uint8_t s_in[BLUR_TH + 6][BLUR_TW + 8];
-  __shared__ float s_row[BLUR_TH + 6][BLUR_TW + 1];
-  int level = 0;
-  while (level + 1 < plan.nlevels && (int)blockIdx.x >= tiles.first[level + 1]) ++level;
-  const int tile = (int)blockIdx.x - tiles.first[level];
-  const OrbLevelDev &L = plan.lv[level];
-  const int f = blockIdx.z, tx0 = (tile % tiles.nx[level]) * BLUR_TW, ty0 = (tile / tiles.nx[level]) * BLUR_TH;
-  const int w = L.w, h = L.h;
-  const uint8_t *img = planes + (size_t)f * plan.slot_bytes + L.img_off;
-  uint8_t *out = planes + (size_t)f * plan.slot_bytes + L.blur_off;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < (BLUR_TH + 6) * (BLUR_TW + 6); i += 256) {
-    const int r = i / (BLUR_TW + 6), c = i - r * (BLUR_TW + 6);
-    int y = ty0 + r - 3, x = tx0 + c - 3;
-    y = y < 0 ? -y : (y >= h ? 2 * h - 2 - y : y);        // BORDER_REFLECT_101
-    x = x < 0 ? -x : (x >= w ? 2 * w - 2 - x : x);
-    y = max(0, min(y, h - 1));
-    x = max(0, min(x, w - 1));
-    s_in[r][c] = img[(size_t)y * L.pitch + x];
-  }
-  __syncthreads();
-  for (int i = tid; i < (BLUR_TH + 6) * BLUR_TW; i += 256) {
-    const int r = i / BLUR_TW, c = i - r * BLUR_TW;
-    float s = __fmul_rn(c_gauss7[0], (float)s_in[r][c]);
-#pragma unroll
-    for (int k = 1; k < 7; ++k) s = __fadd_rn(s, __fmul_rn(c_gauss7[k], (float)s_in[r][c + k]));
-    s_row[r][c] = s;
-  }
-  __syncthreads();
-  for (int i = tid; i < BLUR_TH * (BLUR_TW / 4); i += 256) {
-    const int r = i / (BLUR_TW / 4), c4 = (i - r * (BLUR_TW / 4)) * 4;
-    const int y = ty0 + r;
-    if (y >= h || tx0 + c4 >= L.pitch) continue;
-    uint32_t pk = 0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int c = c4 + j;
-      float s = __fmul_rn(c_gauss7[3], s_row[r + 3][c]);
-#pragma unroll
-      for (int k = 1; k <= 3; ++k)
-        s = __fadd_rn(s, __fmul_rn(c_gauss7[3 + k], __fadd_rn(s_row[r + 3 + k][c], s_row[r + 3 - k][c])));
-      int v = __float2int_rn(s);
-      v = max(0, min(255, v));
-      pk |= (uint32_t)v << (8 * j);
-    }
-    *reinterpret_cast<uint32_t *>(out + (size_t)y * L.pitch + tx0 + c4) = pk;
-  }
-}
+#include "orb_variants.cuh"   // k_blur2, the descriptor blur; host-emulated in tests
 
 // -------------------------------------------------------------------------------- describe
 __device__ __forceinline__ int warp_sum(int v) {
@@ -1249,8 +1198,6 @@ k_describe(OrbPlanDev plan, const uint8_t *__restrict__ planes, const uint2 *__r
   }
 }
 
-#include "orb_variants.cuh"   // k_blur2 (the shipped descriptor blur; MVO_BLUR2=0: k_blur), host-emulated in tests
-
 // Harris response of every compact candidate of the frames whose levels overflow (retainBest needs them all).  One THREAD
 // per candidate: the 9 x 9 neighbourhood is read once into registers, the 49 Sobel-like gradients and the three integer sums
 // follow from it (a warp per candidate spent ~100 instructions on three shuffle reductions for 49 pixels).  Same integer
@@ -1375,7 +1322,7 @@ int orb_launch_pyramid(mvo_ctx *ctx, const OrbPlanDev &plan, const int32_t *tabl
 
 int orb_launch_gray_pyramid(mvo_ctx *ctx, const OrbPlanDev &plan, const uint8_t *d_in, int channels, size_t stride, size_t frame_stride,
                             const int32_t *tables, uint8_t *planes, int batch) {
-  static const bool off = getenv("MVO_PYR_FUSED") != nullptr && atoi(getenv("MVO_PYR_FUSED")) == 0;      // A/B hook
+  static const bool off = getenv("MVO_PYR_FUSED") != nullptr && atoi(getenv("MVO_PYR_FUSED")) == 0;      // test hook: forces the fallback below
   size_t smem = 0;
   for (int l = 0; l + 1 < plan.nlevels; ++l) smem += (size_t)plan.pyr_rows[l] * plan.lv[l].pitch;
   smem += 16;
@@ -1411,7 +1358,7 @@ struct OrbTmaState {
 };
 
 static bool orb_tma_maps(mvo_ctx *ctx, const OrbPlanDev &plan, const uint8_t *planes, int slots, const FastMaps **out) {
-  static const bool off = getenv("MVO_FAST_TMA") != nullptr && atoi(getenv("MVO_FAST_TMA")) == 0;      // A/B hook
+  static const bool off = getenv("MVO_FAST_TMA") != nullptr && atoi(getenv("MVO_FAST_TMA")) == 0;      // test hook: forces the vector-load fallback
   if (off) return false;
   if (!ctx->orb_tma) ctx->orb_tma = new OrbTmaState();
   OrbTmaState *t = (OrbTmaState *)ctx->orb_tma;
@@ -1472,7 +1419,7 @@ int orb_launch_fast(mvo_ctx *ctx, const OrbPlanDev &plan, const uint8_t *planes,
 }
 
 // 1 when the two-pass grid selection (grid_rank_keep_seg) can run: its 32 count tables fit next to `smem` bytes and the per-cell
-// limit stays below the saturation value of a byte counter; MVO_GRID_ROUNDS=1 keeps the round version (A/B hook)
+// limit stays below the saturation value of a byte counter; MVO_GRID_ROUNDS=1 forces the round version (test hook)
 static int orb_seg_tab(size_t smem, int ncell, int max_per_cell) {
   static const bool rounds = getenv("MVO_GRID_ROUNDS") != nullptr && atoi(getenv("MVO_GRID_ROUNDS")) != 0;
   return (!rounds && max_per_cell <= 254 && smem + (size_t)32 * ncell + 32 <= 220 * 1024) ? 1 : 0;
@@ -1505,11 +1452,8 @@ int orb_launch_blur(mvo_ctx *ctx, const OrbPlanDev &plan, uint8_t *planes, int b
   }
   tiles.first[plan.nlevels] = total;
   dim3 grid(total, 1, batch);
-  // k_blur2 (tile moved as words, 4 outputs per thread), byte-identical output to k_blur: default since round 2; MVO_BLUR2=0 = old kernel
-  static const bool use_blur2 = getenv("MVO_BLUR2") == nullptr || atoi(getenv("MVO_BLUR2")) != 0;
   KTimer kt(ctx, KC_BLUR);
-  if (use_blur2) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, dim3(256), 0, k_blur2, plan, tiles, planes));
-  else MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, dim3(256), 0, k_blur, plan, tiles, planes));
+  MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, dim3(256), 0, k_blur2, plan, tiles, planes));
   MVO_CHECK_LAUNCH(ctx);
   return MVO_OK;
 }

@@ -1,14 +1,12 @@
-// k_blur2: the descriptor blur of the shipped path (byte-identical with k_blur, fewer instructions; MVO_BLUR2=0 selects the
-// round-1 kernel).  Kept in a header of its own so that the CPU test tier can compile the very same kernel text for the
-// host and run it thread by thread (tests/cpp/orb_variants_emu.cpp) against the oracle.
+// k_blur2: the descriptor blur.  Kept in a header of its own so that the CPU test tier can compile the very same kernel text
+// for the host and run it thread by thread (tests/cpp/orb_variants_emu.cpp) against the oracle.
 //
 // Included by orb.cu INSIDE its anonymous namespace, after these have been defined there: c_gauss7[7] (the Gaussian taps),
 // BLUR_TW / BLUR_TH, struct BlurTiles and the declarations of orb.cuh.
 #pragma once
 
-// Same filter, same arithmetic (identical operand order, no FMA), fewer instructions: the tile is moved as 32-bit words,
-// the row pass produces four outputs per thread from three shared-memory words, the column pass two rows of four outputs
-// per thread from eight float4 rows.
+// No FMA, the operand order of OpenCV's float filter: the tile is moved as 32-bit words, the row pass produces four outputs
+// per thread from three shared-memory words, the column pass two rows of four outputs per thread from eight float4 rows.
 constexpr int BLUR2_INW = BLUR_TW / 4 + 2;      // input words per tile row: 4-px halo word left and right
 constexpr int BLUR2_ROWF = BLUR_TW + 4;         // floats per row of the row-pass result (16-byte aligned rows, skewed banks)
 

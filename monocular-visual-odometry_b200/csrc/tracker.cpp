@@ -498,8 +498,7 @@ static int submit_extraction(mvo_tracker *t, const uint8_t *image, int channels,
   j.want_host = !use_device_path(t);
   j.rc = MVO_OK; j.nk = 0; j.d_k = nullptr; j.d_d = nullptr;
   j.prematch = false; j.matched = false;
-  static const bool no_prematch = getenv("MVO_TRACK_NO_PREMATCH") != nullptr;      // A/B hook
-  if (!j.want_host && t->prm.match_method != 3 && !no_prematch) {
+  if (!j.want_host && t->prm.match_method != 3) {
     MVO_TRY(dev_alloc(t));                          // the worker needs the device copy of the map
     j.prematch = true;
     j.match_mode = t->prm.match_method == 1 ? 0 : 1;
@@ -747,8 +746,8 @@ int mvo_trk_set_ref_desc(mvo_tracker *t, int slot, int tag) {
 
 // Keyframe insertion, device-resident mode: everything the host needs of the frame that was just tracked, in ONE submission
 // and ONE synchronisation — keypoints, descriptors, colours (gathered on the device for an image in device memory), the
-// connections PnP gave it (inliers_to_mappt_connections_), the visible / matched increments since the last call (reset like
-// mvo_trk_counters does; with_links = 0 for a frame that has not been tracked: initialisation), and the matcher keys of the reference keyframe's descriptors against this frame's (match_mode 0 =
+// connections PnP gave it (inliers_to_mappt_connections_), the visible / matched increments since the last call (read and
+// reset; with_links = 0 for a frame that has not been tracked: initialisation), and the matcher keys of the reference keyframe's descriptors against this frame's (match_mode 0 =
 // nearest neighbour, 1 = two nearest; only when the descriptors kept by mvo_trk_set_ref_desc carry `ref_tag`).
 int mvo_trk_keyframe_fetch(mvo_tracker *t, int slot, int want_rgb, int with_links, int n_counters, int ref_tag, int match_mode, MvoKfFetch *out) {
   mvo_ctx *ctx = t->ctx;
@@ -967,25 +966,6 @@ int mvo_trk_links(mvo_tracker *t, int k, int32_t *ids, int32_t *kp_idx, int cap,
   return MVO_OK;
 }
 
-// MapPoint::visible_times_ / matched_times_ increments since the last call (or map upload), per position in the map arrays
-int mvo_trk_counters(mvo_tracker *t, int32_t *visible, int32_t *matched, int n) {
-  mvo_ctx *ctx = t->ctx;
-  if (n <= 0) return MVO_OK;
-  if (t->dev_nmap < 0) {              // no frame has been tracked against this map yet
-    memset(visible, 0, (size_t)n * 4);
-    memset(matched, 0, (size_t)n * 4);
-    return MVO_OK;
-  }
-  if (n != t->dev_nmap) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "tracker: counters asked for %d points, the device map holds %d", n, t->dev_nmap);
-  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  MVO_CUDA(ctx, cudaMemcpyAsync(visible, t->d_vis_cnt, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(matched, t->d_match_cnt, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaMemsetAsync(t->d_vis_cnt, 0, (size_t)n * 4, ctx->stream));
-  MVO_CUDA(ctx, cudaMemsetAsync(t->d_match_cnt, 0, (size_t)n * 4, ctx->stream));
-  MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return MVO_OK;
-}
-
 // the tracking step of an acquired frame with the caller's guess (reference keyframe) and previous-frame poses
 int mvo_trk_track(mvo_tracker *t, int slot, const double *T_guess, const double *T_prev, double *T_w_c_out, mvo_track_result *res, int ref_k,
                   int allow_spec) {
@@ -1006,7 +986,6 @@ int mvo_trk_track(mvo_tracker *t, int slot, const double *T_guess, const double 
 //   +256: world->camera pose of the frame before BA (12 doubles)      +512: BA statistics (16 doubles)
 static int track_device(mvo_tracker *t, ExtractJob &job, int slot, double *T_w_c_out, mvo_track_result *res, int ref_k, int allow_spec) {
   mvo_ctx *ctx = t->ctx;
-  static const bool spec_off = getenv("MVO_TRACK_SPEC") != nullptr && atoi(getenv("MVO_TRACK_SPEC")) == 0;      // A/B hook
   // ring slot of the reference keyframe (the frame whose pose is the initial guess), looked up before this frame enters the buffer
   int ref_slot = -1;
   if (ref_k >= 1 && ref_k <= (int)t->frames.size()) ref_slot = t->frames[t->frames.size() - (size_t)ref_k].slot;
@@ -1202,7 +1181,7 @@ static int track_device(mvo_tracker *t, ExtractJob &job, int slot, double *T_w_c
     }
     // next frame: its extraction and pre-match run on the worker while this frame is tracked; once they are done its chain head
     // goes into the stream behind this frame's results, with the reference pose read from the ring slot this frame's BA may move
-    if (allow_spec && !spec_off && ref_slot >= 0 && project_in_filter && can_match && prematched && t->n_submit != t->n_consume && rc == MVO_OK) {
+    if (allow_spec && ref_slot >= 0 && project_in_filter && can_match && prematched && t->n_submit != t->n_consume && rc == MVO_OK) {
       speculate = [&, ref_slot]() -> int {
         const int ns = (int)(t->n_consume % MVO_XSLOTS);
         ExtractJob &nj = t->job[ns];

@@ -23,8 +23,9 @@
 //     keyframe changes it), the frame buffer and the BA graph stay in HBM, a tracked frame costs one host synchronisation,
 //     and MapPoint::visible_times_ / matched_times_ are accumulated on the device and read back when optimizeMap_ needs
 //     them.  Keypoints, descriptors and connections of a tracked frame are only copied to the host when the frame becomes
-//     a keyframe (or the caller asks for them).  Initialisation and keyframe insertion run through the host-array entry
-//     points as below: they happen once per sequence / per keyframe.
+//     a keyframe (or the caller asks for them).  Initialisation and keyframe insertion fetch the frame (a keyframe also its
+//     connections and the counters) with its match against the reference keyframe in one synchronisation
+//     (mvo_trk_keyframe_fetch); a keyframe's essential-matrix RANSAC and its triangulation share one submission.
 //   * host arrays (device_resident = 0, and always with free map points): every stage through its public entry point,
 //     four host round trips per tracked frame, as a maintainer who only swaps the bodies of the reference functions gets it.
 // Both give the same states, counts and keyframes; poses agree to the summation order of the BA (tests/test_vo_pipeline_gpu.py).
@@ -161,7 +162,7 @@ struct mvo_vo {
   int cur_channels = 0, cur_on_device = 0;
   size_t cur_stride = 0;
   std::vector<uint8_t> img_scratch;
-  std::vector<int32_t> new_ids, new_kp, cnt_vis, cnt_match;
+  std::vector<int32_t> new_ids, new_kp;
   std::vector<float> new_obs, up_pts, tri_all;
   std::vector<uint8_t> up_desc;
 };
@@ -267,21 +268,6 @@ int upload_map(mvo_vo *v) {
     ++k;
   }
   return mvo_trk_set_map_ids(v->trk, v->up_pts.data(), v->up_desc.data(), v->dev_order.data(), (int)n, 0);
-}
-
-// device-resident mode: fold the visible / matched increments the tracker accumulated since the last upload into the map
-int pull_counters(mvo_vo *v) {
-  const int n = (int)v->dev_order.size();
-  if (n == 0) return MVO_OK;
-  v->cnt_vis.resize((size_t)n); v->cnt_match.resize((size_t)n);
-  MVO_TRY(mvo_trk_counters(v->trk, v->cnt_vis.data(), v->cnt_match.data(), n));
-  for (int k = 0; k < n; ++k) {
-    auto it = v->map_points.find(v->dev_order[(size_t)k]);
-    if (it == v->map_points.end()) continue;
-    it->second.visible_times += v->cnt_vis[(size_t)k];
-    it->second.matched_times += v->cnt_match[(size_t)k];
-  }
-  return MVO_OK;
 }
 
 // the increments of one keyframe fetch (positions = the order of the last upload) folded into the map
@@ -607,9 +593,7 @@ int insert_keyframe(mvo_vo *v, mvo_vo_frame_info *info) {
   StageClock clk;
   const int method = v->prm.track.match_method;
   bool matched = false;
-  static const bool legacy = getenv("MVO_VO_LEGACY_KEYFRAME") != nullptr;      // A/B hook: the stage-by-stage path of round 1
-  const bool fused = v->dev && !legacy;
-  if (fused) {
+  if (v->dev) {
     // the frame's keypoints, descriptors, colours and connections, the visible / matched increments and the match against the
     // reference keyframe (whose descriptors stayed on the device): one submission, one synchronisation
     MvoKfFetch kf;
@@ -630,10 +614,6 @@ int insert_keyframe(mvo_vo *v, mvo_vo_frame_info *info) {
       c.matches_with_ref.resize((size_t)nm);
       matched = true;
     }
-  } else if (v->dev) {                                           // the frame's keypoints and connections come to the host now
-    MVO_TRY(ensure_host(v, &c));
-    MVO_TRY(ensure_conn(v, &c, 0));
-    clk.mark("fetch");
   }
   if (!matched) MVO_TRY(match_into(v, r.desc.data(), r.xy.data(), r.n(), c, method, v->prm.max_match_dist_triangulation, &c.matches_with_ref));
   clk.mark("match");
@@ -656,13 +636,13 @@ int insert_keyframe(mvo_vo *v, mvo_vo_frame_info *info) {
     b[0] = (float)(((double)c.xy[2 * m.train_idx] - v->K[2]) / v->K[0]); b[1] = (float)(((double)c.xy[2 * m.train_idx + 1] - v->K[5]) / v->K[4]);
   };
   // helperFindInlierMatchesByEpipolarCons (motion_estimation.cpp:180-196): the inliers of the essential-matrix RANSAC.  The
-  // reference passes dummy R / t here, so only the consensus set is computed; in the fused path the triangulation of every
+  // reference passes dummy R / t here, so only the consensus set is computed; in device-resident mode the triangulation of every
   // correspondence (its motion is known beforehand) rides in the same submission and the inliers' rows are picked below.
   double E[9], Re[9], te[3];
   v->inl.resize((size_t)n);
   int ni = n;
   int rc;
-  if (fused) {
+  if (v->dev) {
     v->np1.resize((size_t)n * 2); v->np2.resize((size_t)n * 2);
     for (int i = 0; i < n; ++i) to_norm_plane(c.matches_with_ref[(size_t)i], &v->np1[2 * (size_t)i], &v->np2[2 * (size_t)i]);
     v->tri_all.resize((size_t)n * 3);
@@ -681,7 +661,7 @@ int insert_keyframe(mvo_vo *v, mvo_vo_frame_info *info) {
     c.inliers_matches_with_ref[(size_t)i] = m;
   }
   v->pts3d.resize((size_t)std::max(ni, 1) * 3);
-  if (fused) {
+  if (v->dev) {
     for (int i = 0; i < ni; ++i) memcpy(&v->pts3d[3 * (size_t)i], &v->tri_all[3 * (size_t)v->inl[i]], 12);
   } else {
     v->np1.resize((size_t)ni * 2); v->np2.resize((size_t)ni * 2);
@@ -698,8 +678,6 @@ int insert_keyframe(mvo_vo *v, mvo_vo_frame_info *info) {
   v->new_ids.clear(); v->new_kp.clear(); v->new_obs.clear();
   push_curr_points_to_map(v);
   clk.mark("retain+push");
-  if (v->dev && !fused) MVO_TRY(pull_counters(v));               // visible_times_ / matched_times_ as of this frame
-  clk.mark("counters");
   optimize_map(v);
   clk.mark("optimize_map");
   if (v->dev) {
@@ -859,9 +837,8 @@ int mvo_vo_add_frame_ex(mvo_vo *v, const uint8_t *image, int channels, size_t st
   } else if (v->state == VO_DOING_INITIALIZATION) {              // :35-69
     const VoFrame &r = *v->ref;
     bool matched = false;
-    static const bool legacy = getenv("MVO_VO_LEGACY_KEYFRAME") != nullptr;
     const int mi = v->prm.match_method_init;
-    if (v->dev && !legacy) {            // the frame's host copy and its match against the first keyframe in one synchronisation
+    if (v->dev) {                       // the frame's host copy and its match against the first keyframe in one synchronisation
       MvoKfFetch kf;
       rc = mvo_trk_keyframe_fetch(v->trk, slot, v->cur_on_device, 0, 0, r.id, mi == 1 ? 0 : (mi == 2 ? 1 : -1), &kf);
       if (rc == MVO_OK) {
@@ -874,8 +851,6 @@ int mvo_vo_add_frame_ex(mvo_vo *v, const uint8_t *image, int channels, size_t st
           matched = rc == MVO_OK;
         }
       }
-    } else if (v->dev) {
-      rc = ensure_host(v, frame.get());
     }
     if (rc == MVO_OK && !matched)
       rc = match_into(v, r.desc.data(), r.xy.data(), r.n(), *frame, mi, v->prm.max_match_dist_init, &frame->matches_with_ref);

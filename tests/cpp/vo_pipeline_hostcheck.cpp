@@ -156,5 +156,4 @@ int mvo_trk_set_map_ids(mvo_tracker *, const float *, const uint8_t *, const int
 int mvo_trk_push_frame(mvo_tracker *, const double *, const int32_t *, const int32_t *, const float *, int) { return MVO_ERR_UNSUPPORTED; }
 int mvo_trk_append_links(mvo_tracker *, int, const int32_t *, const int32_t *, const float *, int) { return MVO_ERR_UNSUPPORTED; }
 int mvo_trk_links(mvo_tracker *, int, int32_t *, int32_t *, int, int *) { return MVO_ERR_UNSUPPORTED; }
-int mvo_trk_counters(mvo_tracker *, int32_t *, int32_t *, int) { return MVO_ERR_UNSUPPORTED; }
 int mvo_trk_track(mvo_tracker *, int, const double *, const double *, double *, mvo_track_result *, int, int) { return MVO_ERR_UNSUPPORTED; }

@@ -2,8 +2,8 @@
 (tests/emu_build.py: kernels through tests/cpp/cuda_emu.h, one OS thread per CUDA thread; the CUDA runtime calls of the host
 code through tests/emu/cuda_runtime_emu.cpp) — the real host orchestration and every ORB kernel — against the numpy
 restatement of cv::ORB + selectUniformKptsByGrid (oracle/, pinned against cv2): keypoints and descriptors bit-exact, like the
-hardware test tests/test_orb_gpu.py, on small images.  Also run with the kernels of round 1 switched back on
-(MVO_BLUR2 / MVO_PYR_FUSED / MVO_GRID_ROUNDS select the kernels the shipped path replaced; separate processes: the switches are read once)."""
+hardware test tests/test_orb_gpu.py, on small images.  Also run with the geometry fallbacks forced on (MVO_PYR_FUSED /
+MVO_GRID_ROUNDS select the kernels that very wide images and high per-cell limits take; separate processes: the switches are read once)."""
 import os
 import subprocess
 import sys
@@ -27,8 +27,8 @@ cases = [(mvo_synth.gray_to_bgr(mvo_synth.rect_scene(3, 320, 240, n_rect=300)), 
          # device (k_retain: warp-level and CTA-level partitions), then the grid selection over the retained order (k_select_kept)
          (mvo_synth.rect_scene(4, 200, 152, n_rect=120), 120, 300), (mvo_synth.noise_scene(2, 256, 200), 900, 2000)]
 import os
-if os.environ.get("MVO_BLUR2", "1") == "0":
-    cases = cases[1:3]                     # the replaced kernels: the smaller image only (run time)
+if os.environ.get("MVO_PYR_FUSED", "1") == "0":
+    cases = cases[1:3]                     # the fallback kernels: the smaller image only (run time)
 lib.mvo_test_orb_host_fallbacks.restype = C.c_uint64
 for img, cap, nfeat in cases:
     p = mvo_b200.Params()
@@ -50,7 +50,7 @@ print("orb emu child ok")
 '''
 
 
-@pytest.mark.parametrize("env", [{"MVO_BLUR2": "1"}, {"MVO_BLUR2": "0", "MVO_PYR_FUSED": "0", "MVO_GRID_ROUNDS": "1"}], ids=["shipped", "round1_kernels"])
+@pytest.mark.parametrize("env", [{}, {"MVO_PYR_FUSED": "0", "MVO_GRID_ROUNDS": "1"}], ids=["shipped", "geometry_fallbacks"])
 def test_emulated_orb_extraction_is_bit_exact(tmp_path, env):
     e = dict(os.environ)
     e.update(env)

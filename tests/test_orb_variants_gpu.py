@@ -1,7 +1,8 @@
-"""The kernels the shipped ORB path replaced stay selectable (MVO_BLUR2=0: k_blur; MVO_PYR_FUSED=0: k_gray + k_resize; MVO_FAST_TMA=0:
-vector-load staging; MVO_GRID_ROUNDS=1: round-based grid selection; MVO_PDL=0: plain launches).  The switches are read once per
-process, so each configuration runs in its own child process; keypoints and descriptors must be byte-identical with the shipped
-kernels' (which are themselves bit-exact with cv2, tests/test_orb_gpu.py)."""
+"""The geometry fallbacks of the ORB path, forced on ordinary scenes (MVO_PYR_FUSED=0: k_gray + k_resize, taken for very wide images
+with many levels; MVO_FAST_TMA=0: vector-load staging, taken above 1024 px; MVO_GRID_ROUNDS=1: round-based grid selection, taken above
+254 points per cell; MVO_PDL=0: plain launches).  The switches are read once per process, so each configuration runs in its own child
+process; keypoints and descriptors must be byte-identical with the default kernels' (which are themselves bit-exact with cv2,
+tests/test_orb_gpu.py)."""
 import os
 import subprocess
 import sys
@@ -45,7 +46,7 @@ def _extract(tmp_path, name, env):
     return np.load(out)
 
 
-@pytest.mark.parametrize("env", [{"MVO_BLUR2": "0"}, {"MVO_PYR_FUSED": "0", "MVO_FAST_TMA": "0", "MVO_GRID_ROUNDS": "1", "MVO_PDL": "0"}], ids=["round1_blur", "round1_pyramid_fast_select"])
+@pytest.mark.parametrize("env", [{"MVO_PYR_FUSED": "0", "MVO_FAST_TMA": "0", "MVO_GRID_ROUNDS": "1", "MVO_PDL": "0"}], ids=["geometry_fallbacks"])
 def test_variant_is_byte_identical_with_the_shipped_kernels(built, tmp_path, env):
     ref = _extract(tmp_path, "shipped", {})
     got = _extract(tmp_path, "variant", env)

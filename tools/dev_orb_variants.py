@@ -1,4 +1,4 @@
-"""Timing of the experimental ORB kernel variants against the shipped ones: batched device-resident extraction (64 frames
+"""Timing of the ORB geometry fallbacks (and of plain launches) against the default kernels: batched device-resident extraction (64 frames
 per call, as bench.py's orb_batch entry) per kernel class.  The switches are read once per process, so this script
 re-executes itself once per configuration.  Usage: python tools/dev_orb_variants.py  -> one JSON line per configuration."""
 import json
@@ -8,7 +8,7 @@ import sys
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-CONFIGS = [{}, {"MVO_BLUR2": "0"}, {"MVO_PYR_FUSED": "0"}, {"MVO_FAST_TMA": "0"}, {"MVO_GRID_ROUNDS": "1"}, {"MVO_PDL_ORB": "0"}]
+CONFIGS = [{}, {"MVO_PYR_FUSED": "0"}, {"MVO_FAST_TMA": "0"}, {"MVO_GRID_ROUNDS": "1"}, {"MVO_PDL_ORB": "0"}]
 
 
 def child():
@@ -48,7 +48,7 @@ def child():
     for it in range(2):
         call((it % 2) * B)
     ms, cnt = mvo_b200.timing_read(ctx)
-    print(json.dumps({"config": {k: v for k, v in os.environ.items() if k in ("MVO_BLUR2", "MVO_PYR_FUSED", "MVO_FAST_TMA", "MVO_GRID_ROUNDS", "MVO_PDL_ORB")}, "us_per_frame": us / B,
+    print(json.dumps({"config": {k: v for k, v in os.environ.items() if k in ("MVO_PYR_FUSED", "MVO_FAST_TMA", "MVO_GRID_ROUNDS", "MVO_PDL_ORB")}, "us_per_frame": us / B,
                       "frames_per_s": B / (us * 1e-6), "kernel_us_per_frame": {names[k]: round(1e3 * ms[k] / (2 * B), 3) for k in range(len(names)) if cnt[k]},
                       "checksum": int(d_d.to(torch.int64).sum().item())}))
 
