@@ -598,6 +598,17 @@ __device__ __forceinline__ double fast_rsqrt(double c) {
   y = y * (1.5 - 0.5 * c * y * y);
   return y;
 }
+// The float seed is 0 or inf outside the float range (rsqrtf(inf) = 0, __frcp_rn(inf) = 0, the seed of a subnormal depth is
+// inf and the Newton steps turn it into -inf or NaN), so a value the LM does not bound takes the exact fp64 operation outside
+// [1e-30, 1e30], as chol6_solve does for its pivots.  A point next to a camera's principal plane (depth below ~1e-17 f |x|)
+// has chi2 above FLT_MAX; g2o weights it by delta / sqrt(chi2) like any other edge.
+__device__ __forceinline__ double ranged_rcp(double z) {
+  const double m = fabs(z);
+  return (m > 1e-30 && m < 1e30) ? fast_rcp(z) : 1.0 / z;
+}
+__device__ __forceinline__ double ranged_rsqrt(double c) {
+  return (c > 1e-30 && c < 1e30) ? fast_rsqrt(c) : 1.0 / sqrt(c);
+}
 
 __device__ __forceinline__ bool chol6_solve(const double *h /*21 packed upper*/, const double *g, double lambda, double *x) {
   // Cholesky with reciprocal diagonal (one rsqrt per column, no divisions on the dependent chain)
@@ -655,14 +666,14 @@ __device__ __forceinline__ void edge_terms(const PoseArgs &a, const double *Rt, 
   const double x = Rt[0] * X0 + Rt[1] * X1 + Rt[2] * X2 + Rt[9];
   const double y = Rt[3] * X0 + Rt[4] * X1 + Rt[5] * X2 + Rt[10];
   const double z = Rt[6] * X0 + Rt[7] * X1 + Rt[8] * X2 + Rt[11];
-  const double iz = fast_rcp(z);
+  const double iz = ranged_rcp(z);
   const double xz = x * iz, yz = y * iz;
   const double e0r = ou - (a.fx * xz + a.cx), e1r = ov - (a.fy * yz + a.cy);
   const double Oe0 = a.i00 * e0r + a.i01 * e1r, Oe1 = a.i10 * e0r + a.i11 * e1r;
   const double chi = e0r * Oe0 + e1r * Oe1;
   double w = 1.0, rho = chi;
   if (a.use_huber && chi > a.huber * a.huber) {     // RobustKernelHuber: rho = 2 sqrt(chi) d - d^2, rho' = d / sqrt(chi)
-    const double ys = fast_rsqrt(chi);
+    const double ys = ranged_rsqrt(chi);
     w = a.huber * ys;
     rho = 2 * (chi * ys) * a.huber - a.huber * a.huber;
   }
@@ -1062,7 +1073,7 @@ __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
         scale += s_fscale[b][f];
         mstep = fmax(mstep, s_fstep[b][f]);
       }
-      const double rscale = fast_rcp(scale + 1e-3);
+      const double rscale = ranged_rcp(scale + 1e-3);
       tiny = a.step_tol > 0 && ok && mstep < a.step_tol;
       const double chi_f = gather(s_new);
       PF_MARK(2);
@@ -1199,6 +1210,60 @@ int mvo_ba_pose_store_launch(mvo_ctx *ctx, const MvoPoseStore &st, int e_upper, 
   return pose_launch(ctx, kern, a, csz, smem);
 }
 
+// Test entry (not part of the C ABI): the device-resident pose LM on a frame buffer given as host arrays.  Uploads them, runs
+// mvo_ba_pose_store_launch as the tracker does, waits, and returns the whole ring of poses (ring x 12, in/out), out_info[0..17]
+// and the 16 stats (both in/out: entries the kernel does not write keep the caller's values).  nslots may exceed 16 to reach
+// the launcher's check; only the first 16 slots are copied.
+extern "C" int mvo_test_ba_pose_store(mvo_ctx *ctx, const float *map_pts, const uint8_t *alive, int n_ids, const int32_t *edge_map,
+                                      const float *edge_obs, const int32_t *cnt, double *pose, int ring, int cap, const int32_t *slots,
+                                      int nslots, int min_links, int skip_flag, int e_upper, const double *K, const double *info,
+                                      int iters, int use_huber, double huber, double step_tol, int32_t *out_info, double *stats) {
+  if (!ctx || !map_pts || !alive || !edge_map || !edge_obs || !cnt || !pose || !slots || !K || !info || !out_info || !stats)
+    return MVO_ERR_INVALID_ARG;
+  if (n_ids < 0 || ring < 1 || cap < 1 || nslots < 0) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "pose BA test: bad sizes");
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t nrc = (size_t)ring * cap;
+  size_t o = 0;
+  const size_t o_map = o;  o = al(o + (size_t)n_ids * 12 + 12);
+  const size_t o_alv = o;  o = al(o + (size_t)n_ids + 1);
+  const size_t o_em = o;   o = al(o + nrc * 4);
+  const size_t o_eo = o;   o = al(o + nrc * 8);
+  const size_t o_cnt = o;  o = al(o + (size_t)ring * 4);
+  const size_t o_pose = o; o = al(o + (size_t)ring * 96);
+  const size_t o_flag = o; o = al(o + 4);
+  const size_t o_info = o; o = al(o + 18 * 4);
+  const size_t o_st = o;   o = al(o + 16 * 8);
+  MVO_TRY(mvo_reserve(ctx, ctx->ba_buf, o));
+  uint8_t *d = (uint8_t *)ctx->ba_buf.p;
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_map, map_pts, (size_t)n_ids * 12, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_alv, alive, (size_t)n_ids, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_em, edge_map, nrc * 4, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_eo, edge_obs, nrc * 8, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_cnt, cnt, (size_t)ring * 4, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_pose, pose, (size_t)ring * 96, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_flag, &skip_flag, 4, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_info, out_info, 18 * 4, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_st, stats, 16 * 8, cudaMemcpyHostToDevice, ctx->stream));
+  MvoPoseStore st;
+  memset(&st, 0, sizeof st);
+  st.map_pts = (const float *)(d + o_map); st.alive = d + o_alv; st.n_ids = n_ids;
+  st.edge_map = (const int32_t *)(d + o_em); st.edge_obs = (const float2 *)(d + o_eo); st.cnt = (const int32_t *)(d + o_cnt);
+  st.pose = (double *)(d + o_pose); st.cap = cap; st.nslots = nslots; st.min_links = min_links;
+  for (int k = 0; k < nslots && k < 16; ++k) st.slot[k] = slots[k];
+  st.skip_flag = (const int32_t *)(d + o_flag); st.out_info = (int32_t *)(d + o_info);
+  // fy = fx, as the tracker passes it (g2o_ba.cpp ignores fy)
+  const int rc = mvo_ba_pose_store_launch(ctx, st, e_upper, K[0], K[0], K[2], K[5], info, iters, use_huber, huber, step_tol,
+                                          (double *)(d + o_st));
+  MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));      // the uploads above are done with the host arrays on every path
+  if (rc != MVO_OK) return rc;
+  MVO_CUDA(ctx, cudaMemcpyAsync(pose, d + o_pose, (size_t)ring * 96, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(out_info, d + o_info, 18 * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(stats, d + o_st, 16 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MVO_OK;
+}
+
 // g2o_ba.cpp:183-190: camera->world T_w_c (4x4 row-major) -> world->camera [R|t] = (T_w_c)^-1 (R row-major, then t)
 static void T_w_c_to_Rt(const double *T, double *q) {
   for (int i = 0; i < 3; ++i) {
@@ -1288,9 +1353,10 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
     for (int f = 0; f < F; ++f) Rt_to_T_w_c(hpose + 12 * f, poses_T_w_c + 16 * f);
     if (stats) memcpy(stats, h_stats, 32);
     if (getenv("MVO_BA_DEBUG"))
-      fprintf(stderr, "k_ba_pose: F=%d E=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f | "
-              "pdl_wait=%.0f setup=%.0f init=%.0f exit=%.0f kernel=%.0f\n", F, E, h_stats[2], h_stats[15], h_stats[7], h_stats[8], h_stats[9],
-              h_stats[10], h_stats[11], h_stats[12], h_stats[4], h_stats[5], h_stats[6], h_stats[13]);
+      fprintf(stderr, "k_ba_pose: F=%d E=%d Ep=%d chunk=%d cluster=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f "
+              "gather=%.0f decide=%.0f | pdl_wait=%.0f setup=%.0f init=%.0f exit=%.0f kernel=%.0f\n", F, E, Ep, chunk, csz, h_stats[2],
+              h_stats[15], h_stats[7], h_stats[8], h_stats[9], h_stats[10], h_stats[11], h_stats[12], h_stats[4], h_stats[5], h_stats[6],
+              h_stats[13]);
     return MVO_OK;
   }
 

@@ -12,7 +12,9 @@
 
 #include "pdl_device.cuh"
 
-// grid x block threads, `cluster` CTAs per cluster (1 = no cluster attribute)
+// grid x block threads, `cluster` CTAs per cluster (0 = no cluster attribute).  A kernel that uses cluster instructions (distributed
+// shared memory, st.async, cluster barriers) needs the attribute even for a cluster of one CTA: without it the first of them faults
+// with an illegal instruction.
 template <class... P, class... A>
 static inline cudaError_t launch_pdl(cudaStream_t stream, unsigned grid, unsigned block, size_t smem, unsigned cluster, void (*kernel)(P...), A &&...args) {
   static const bool pdl_on = !(getenv("MVO_PDL") && atoi(getenv("MVO_PDL")) == 0);
@@ -23,7 +25,7 @@ static inline cudaError_t launch_pdl(cudaStream_t stream, unsigned grid, unsigne
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   unsigned na = 0;
-  if (cluster > 1) {
+  if (cluster > 0) {
     attr[na].id = cudaLaunchAttributeClusterDimension;
     attr[na].val.clusterDim.x = cluster;
     attr[na].val.clusterDim.y = 1;

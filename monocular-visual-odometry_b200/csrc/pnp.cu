@@ -125,18 +125,18 @@ static int pnp_enqueue(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, c
   if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "solvePnPRansac: more than %d correspondences", 200 * 1024 / 20);
   const double thr2 = (double)ctx->prm.pnp_reproj_error * (double)ctx->prm.pnp_reproj_error;
   { KTimer kt(ctx, KC_PNP_HYP);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)((H + 127) / 128), 128, 0, 1, k_pnp_hypotheses, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam,
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)((H + 127) / 128), 128, 0, 0, k_pnp_hypotheses, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam,
                            (uint64_t)ctx->prm.pnp_seed, H, w.poses, w.valid)); }
   ctx->launches++;
   if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_pnp_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (H + 7) / 8;                                   // one hypothesis per warp while the CTAs of one wave allow it
   if (grid > 4 * ctx->sm_count) grid = 4 * ctx->sm_count;
   { KTimer kt(ctx, KC_PNP_SCORE);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)grid, 256, smem, 1, k_pnp_score, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)grid, 256, smem, 0, k_pnp_score, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
                            (const double *)w.poses, (const int32_t *)w.valid, w.counts)); }
   ctx->launches++;
   { KTimer kt(ctx, KC_PNP_FINISH);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, FIN_T, 0, 1, k_pnp_finish, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, FIN_T, 0, 0, k_pnp_finish, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
                            (const double *)w.poses, (const int32_t *)w.counts, 0, (int)ctx->prm.pnp_refine_iters, w.pose_io, w.out_i, w.inl, w.ex, w.eo, w.ef)); }
   ctx->launches++;
   ctx->pnp_last_h = H;

@@ -203,7 +203,7 @@ int mvo_track_glue(mvo_ctx *ctx, const MvoTrackGlue &g) {
   a.map_ids = g.map_ids; a.vis = g.vis; a.nmap = g.nmap; a.vis_cnt = g.vis_cnt; a.match_cnt = g.match_cnt;
   a.skip_flag = g.skip_flag; a.res_i = g.res_i; a.res_d = g.res_d;
   KTimer kt(ctx, KC_TRACK);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, 1024, 0, 1, k_track_glue, a));
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, 1024, 0, 0, k_track_glue, a));
   ctx->launches++;
   return MVO_OK;
 }
@@ -257,7 +257,7 @@ int mvo_track_match_filter(mvo_ctx *ctx, const MvoTrackFilter &f) {
   const size_t smem = (size_t)cap * (4 + 4 + 2 + 2 + 2) + 3 * ((size_t)cap / 16 + 2) * 4 + ((size_t)cap / 16 + 2) + 64;
   MVO_CUDA(ctx, cudaFuncSetAttribute(k_match_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   KTimer kt(ctx, KC_TRACK);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, MF_T, smem, 1, k_match_filter, a));
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, MF_T, smem, 0, k_match_filter, a));
   ctx->launches++;
   return MVO_OK;
 }
