@@ -100,13 +100,34 @@ static int pnp_refit(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam) {
 // w.p3 / w.p2 hold the n correspondences on the device
 static int pnp_hyp_count(const mvo_ctx *ctx) { return ctx->prm.pnp_mode == 1 ? 100 : ctx->prm.pnp_hypotheses; }   // vo.cpp:315: iterationsCount = 100
 
+// The hypotheses of either mode into w.poses / w.valid: P3P on counter-based samples (pnp_mode = 0), or the EPnP poses of
+// cv::solvePnPRansac's 100 iterations (pnp_mode = 1, pnp_cv_kernels.cuh).
+static int pnp_enqueue_hypotheses(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, const int32_t *n_dev) {
+  const int H = pnp_hyp_count(ctx);
+  if (ctx->prm.pnp_mode == 1) {
+    { KTimer kt(ctx, KC_PNP_HYP);
+    k_pnp_epnp<<<(H + CVP_WARPS - 1) / CVP_WARPS, CVP_WARPS * 32, 0, ctx->stream>>>(w.p3, w.p2, n, n_dev, cam, H, w.poses, w.valid); }
+    MVO_CHECK_LAUNCH(ctx);
+    return MVO_OK;
+  }
+  { KTimer kt(ctx, KC_PNP_HYP);
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)((H + 127) / 128), 128, 0, 0, k_pnp_hypotheses, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam,
+                           (uint64_t)ctx->prm.pnp_seed, H, w.poses, w.valid)); }
+  ctx->launches++;
+  return MVO_OK;
+}
+
+// The scoring kernel of pnp_mode = 0 stages the n correspondences in shared memory (20 bytes each)
+static int pnp_check_size(mvo_ctx *ctx, int n) {
+  if (ctx->prm.pnp_mode != 1 && (size_t)n * 5 * sizeof(float) > 200 * 1024)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "solvePnPRansac: more than %d correspondences", 200 * 1024 / 20);
+  return MVO_OK;
+}
+
 // pnp_mode = 1: cv::solvePnPRansac's own flow (pnp_cv_kernels.cuh) — 100 EPnP iterations evaluated in parallel, the adaptive loop replayed
-static int pnp_enqueue_cv(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, const int32_t *n_dev) {
+static int pnp_score_finish_cv(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, const int32_t *n_dev) {
   const int H = pnp_hyp_count(ctx);
   const double thr2 = (double)ctx->prm.pnp_reproj_error * (double)ctx->prm.pnp_reproj_error;
-  { KTimer kt(ctx, KC_PNP_HYP);
-  k_pnp_epnp<<<(H + CVP_WARPS - 1) / CVP_WARPS, CVP_WARPS * 32, 0, ctx->stream>>>(w.p3, w.p2, n, n_dev, cam, H, w.poses, w.valid); }
-  MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_PNP_SCORE);
   k_pnp_score_cv<<<(H + 7) / 8, 256, 0, ctx->stream>>>(w.p3, w.p2, n, n_dev, cam, (float)thr2, H, w.poses, w.valid, w.counts); }
   MVO_CHECK_LAUNCH(ctx);
@@ -118,17 +139,15 @@ static int pnp_enqueue_cv(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam
   return pnp_refit(ctx, w, n, cam);
 }
 
-static int pnp_enqueue(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, const int32_t *n_dev = nullptr) {
-  if (ctx->prm.pnp_mode == 1) return pnp_enqueue_cv(ctx, w, n, cam, n_dev);
+// scores -> consensus set of the best hypothesis -> least-squares refit, on the hypotheses in w.poses / w.valid
+static int pnp_score_finish(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, const int32_t *n_dev) {
+  if (ctx->prm.pnp_mode == 1) return pnp_score_finish_cv(ctx, w, n, cam, n_dev);
+  MVO_TRY(pnp_check_size(ctx, n));
   const int H = ctx->prm.pnp_hypotheses;
   const size_t smem = (size_t)n * 5 * sizeof(float);
-  if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "solvePnPRansac: more than %d correspondences", 200 * 1024 / 20);
   const double thr2 = (double)ctx->prm.pnp_reproj_error * (double)ctx->prm.pnp_reproj_error;
-  { KTimer kt(ctx, KC_PNP_HYP);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)((H + 127) / 128), 128, 0, 0, k_pnp_hypotheses, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam,
-                           (uint64_t)ctx->prm.pnp_seed, H, w.poses, w.valid)); }
-  ctx->launches++;
-  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_pnp_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // the 48 KB default covers static and dynamic shared memory together: k_pnp_score's own s_wmax[8] counts as well
+  if (smem + 8 * sizeof(float) > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_pnp_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (H + 7) / 8;                                   // one hypothesis per warp while the CTAs of one wave allow it
   if (grid > 4 * ctx->sm_count) grid = 4 * ctx->sm_count;
   { KTimer kt(ctx, KC_PNP_SCORE);
@@ -145,6 +164,12 @@ static int pnp_enqueue(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, c
   return pnp_refit(ctx, w, n, cam);
 }
 
+static int pnp_enqueue(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &cam, const int32_t *n_dev = nullptr) {
+  MVO_TRY(pnp_check_size(ctx, n));
+  MVO_TRY(pnp_enqueue_hypotheses(ctx, w, n, cam, n_dev));
+  return pnp_score_finish(ctx, w, n, cam, n_dev);
+}
+
 // Device-resident entry points for the tracker (tracker.cpp): reserve the workspace for n correspondences
 // (the caller gathers them into *p3 / *p2 on ctx->stream), then enqueue the whole solvePnPRansac replacement.
 // Results stay on the device: pose_io = [R|t] world->camera after the refit, out_i[0] = consensus-set size
@@ -156,14 +181,55 @@ int mvo_pnp_dev_buffers(mvo_ctx *ctx, int n, float **p3, float **p2, double **po
   return MVO_OK;
 }
 
-// n = number of correspondences, or their upper bound when d_n (device counter) is given
-int mvo_pnp_dev_run(mvo_ctx *ctx, int n, const double *K, const int32_t *d_n) {
+// n = number of correspondences, or their upper bound when d_n (device counter) is given.  own_hypotheses = false scores
+// the hypotheses already in the workspace (mvo_test_pnp_dev).
+static int pnp_dev_run(mvo_ctx *ctx, int n, const double *K, const int32_t *d_n, bool own_hypotheses) {
   if (n < 4) return mvo_fail(ctx, MVO_ERR_DEGENERATE, "solvePnPRansac: %d correspondences (< 4)", n);
   PnpCam cam;
   MVO_TRY(pnp_cam(ctx, K, &cam));
   PnpWs w;
   MVO_TRY(pnp_ws(ctx, n, pnp_hyp_count(ctx), &w));
-  return pnp_enqueue(ctx, w, n, cam, d_n);
+  return own_hypotheses ? pnp_enqueue(ctx, w, n, cam, d_n) : pnp_score_finish(ctx, w, n, cam, d_n);
+}
+
+int mvo_pnp_dev_run(mvo_ctx *ctx, int n, const double *K, const int32_t *d_n) { return pnp_dev_run(ctx, n, K, d_n, true); }
+
+// Test entry (not part of the C ABI): the device-resident PnP as the tracker runs it.  Uploads n_upper correspondences and
+// the device count (any value: the kernels clamp it to n_upper), optionally H = pnp_hypotheses caller-supplied hypotheses
+// (poses H x 12, valid H; pnp_mode = 0 only) in place of k_pnp_hypotheses, runs mvo_pnp_dev_run's sequence with that count,
+// waits, and returns pose_io[12], out_i[4], the inlier list inl[n_upper] and the H scores (counts, -1 = invalid).
+extern "C" int mvo_test_pnp_dev(mvo_ctx *ctx, const float *pts3d, const float *pts2d, int n_upper, int count, const double *K,
+                                const double *poses, const int32_t *valid, double *pose_io, int32_t *out_i, int32_t *inl,
+                                int32_t *counts) {
+  if (!ctx || !pts3d || !pts2d || !K || !pose_io || !out_i || !inl || !counts || (!poses) != (!valid)) return MVO_ERR_INVALID_ARG;
+  if (poses && ctx->prm.pnp_mode == 1) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "pnp test: supplied hypotheses need pnp_mode 0");
+  if (n_upper < 4) return mvo_fail(ctx, MVO_ERR_DEGENERATE, "solvePnPRansac: %d correspondences (< 4)", n_upper);
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int H = pnp_hyp_count(ctx);
+  float *d_p3, *d_p2;
+  double *d_pose;
+  int32_t *d_out, *d_inl;
+  MVO_TRY(mvo_pnp_dev_buffers(ctx, n_upper, &d_p3, &d_p2, &d_pose, &d_out, &d_inl));
+  PnpWs w;
+  MVO_TRY(pnp_ws(ctx, n_upper, H, &w));
+  MVO_TRY(mvo_reserve(ctx, ctx->ba_buf, 256));
+  int32_t *d_n = (int32_t *)ctx->ba_buf.p;
+  MVO_CUDA(ctx, cudaMemcpyAsync(d_p3, pts3d, (size_t)n_upper * 12, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d_p2, pts2d, (size_t)n_upper * 8, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d_n, &count, 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (poses) {
+    MVO_CUDA(ctx, cudaMemcpyAsync(w.poses, poses, (size_t)H * 96, cudaMemcpyHostToDevice, ctx->stream));
+    MVO_CUDA(ctx, cudaMemcpyAsync(w.valid, valid, (size_t)H * 4, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  const int rc = pnp_dev_run(ctx, n_upper, K, d_n, !poses);
+  MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));      // the uploads above are done with the host arrays on every path
+  if (rc != MVO_OK) return rc;
+  MVO_CUDA(ctx, cudaMemcpyAsync(pose_io, d_pose, 96, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(out_i, d_out, 16, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(inl, d_inl, (size_t)n_upper * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(counts, w.counts, (size_t)H * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return MVO_OK;
 }
 
 extern "C" {
