@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
   const int per = (a.P + (int)csize - 1) / (int)csize;
   const int p0 = min((int)rank * per, a.P), p1 = min(p0 + per, a.P);
   double chi_init = 0;
-  int it = 0;
+  int it = 0, rejected = 0;
   bool terminate = false;
   long long ph[8] = {0, 0, 0, 0, 0, 0, 0, 0};     // cycles per phase (thread 0), debug only
   long long tmark = clock64();
@@ -495,10 +495,13 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
           temp += *cluster.map_shared_rank(s_partE + 0, r);
           scale += *cluster.map_shared_rank(s_partE + 1, r);
         }
-        for (int i = 0; i < n; ++i) {
-          const int f = s_act[i / 6];
-          scale += s_dp[i] * (lambda * s_dp[i] + s_full[f * 27 + 21 + i % 6]);
-        }
+        // a failed solve adds nothing (as g2o): its step is zero, but a pose row's b can be NaN (a point at zero depth), and
+        // 0 * NaN would turn the gain ratio into a rejection
+        if (ok)
+          for (int i = 0; i < n; ++i) {
+            const int f = s_act[i / 6];
+            scale += s_dp[i] * (lambda * s_dp[i] + s_full[f * 27 + 21 + i % 6]);
+          }
         if (!ok) temp = 1.7976931348623157e308;
         const double cur = s_ctl[2];
         double r_ = (cur - temp) / (scale + 1e-3);
@@ -522,6 +525,8 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
         for (int i = tid; i < F * 12; i += BA_T) s_pose[i] = s_try[i];
         __syncthreads();
         if (tid == 0) s_ctl[6] = (s_ctl[6] != 0) ? 0.0 : 1.0;
+      } else {
+        ++rejected;
       }
       __syncthreads();
       ++qmax;
@@ -539,6 +544,7 @@ __global__ void __launch_bounds__(BA_T, 1) k_ba(BaArgs a) {
     if (tid == 0) {
       a.stats[0] = chi_init; a.stats[1] = s_ctl[2]; a.stats[2] = it; a.stats[3] = s_ctl[0];
       a.pts_sel[0] = s_ctl[6] != 0 ? 1 : 0;
+      a.stats[7] = rejected;
       for (int q = 0; q < 8; ++q) a.stats[8 + q] = (double)ph[q];
     }
   }
@@ -1415,7 +1421,8 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
   a.pt_start = (const int32_t *)(d + o_start); a.e_frame = (const int32_t *)(d + o_fr); a.obs = (const double *)(d + o_obs);
   a.poses = (double *)(d + o_pose); a.pts_a = (double *)(d + o_pa); a.pts_b = (double *)(d + o_pb);
   a.Hll = (double *)(d + o_hll); a.bl = (double *)(d + o_bl); a.Hinv = (double *)(d + o_hinv); a.Wd = (double *)(d + o_wd);
-  a.stats = (double *)(d + o_stats); a.pts_sel = (int32_t *)(d + o_stats + 32);   // stats[8..15]: phase cycles (debug)
+  // stats[7]: rejected trials, stats[8..15]: phase cycles and trials (debug)
+  a.stats = (double *)(d + o_stats); a.pts_sel = (int32_t *)(d + o_stats + 32);
   // staging chunk for the Schur products: <= 64 KB of shared memory
   int pc = (int)(65536 / ((size_t)F * 36 * 8 + 24));
   pc = std::max(1, std::min(pc, 64));
@@ -1455,8 +1462,9 @@ static int run_ba(mvo_ctx *ctx, double *poses_T_w_c, int F, float *points, int P
   for (int f = 0; f < F; ++f) Rt_to_T_w_c(h_pose + 12 * f, poses_T_w_c + 16 * f);
   if (stats) memcpy(stats, h_stats, 32);
   if (getenv("MVO_BA_DEBUG")) {
-    fprintf(stderr, "k_ba: F=%d P=%d E=%d it=%.0f trials=%.0f cycles A=%.0f B=%.0f C=%.0f D=%.0f E=%.0f F=%.0f sync=%.0f\n", F, P, E,
-            h_stats[2], h_stats[15], h_stats[8], h_stats[9], h_stats[10], h_stats[11], h_stats[12], h_stats[13], h_stats[14]);
+    fprintf(stderr, "k_ba: F=%d P=%d E=%d pc=%d per=%d nact=%d smem=%zu it=%.0f trials=%.0f rejected=%.0f cycles A=%.0f B=%.0f C=%.0f "
+            "D=%.0f E=%.0f F=%.0f sync=%.0f\n", F, P, E, pc, (P + BA_CLUSTER - 1) / BA_CLUSTER, nact, smem, h_stats[2], h_stats[15],
+            h_stats[7], h_stats[8], h_stats[9], h_stats[10], h_stats[11], h_stats[12], h_stats[13], h_stats[14]);
   }
   return MVO_OK;
 }

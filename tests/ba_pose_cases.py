@@ -218,7 +218,7 @@ def parse_debug(text):
 CHILD = r'''
 import json, sys
 sys.path[:0] = [{root!r}, {tests!r}, {py!r}]
-import mvo_b200, ba_pose_cases as B
+import mvo_b200, {module} as B
 ctx = mvo_b200.Context(0)
 for name in {names!r}:
     sys.stderr.write("@case " + name + "\n"); sys.stderr.flush()
@@ -228,16 +228,18 @@ print("child ok")
 '''
 
 
-def run_children(names, cluster=None, lib=None, timeout=1800):
-    """Runs the named cases in one child process (MVO_BA_CLUSTER = cluster, MVO_LIB = lib when given, MVO_BA_DEBUG on);
-    returns {name: (result, [debug records])}."""
+def run_children(names, cluster=None, lib=None, timeout=1800, module="ba_pose_cases"):
+    """Runs the named cases of module (its CASES, run_case and parse_debug) in one child process (MVO_BA_CLUSTER = cluster,
+    MVO_LIB = lib when given, MVO_BA_DEBUG on); returns {name: (result, [debug records])}."""
+    import importlib
+    parse = importlib.import_module(module).parse_debug
     env = dict(os.environ, MVO_BA_DEBUG="1")
     env.pop("MVO_BA_CLUSTER", None)
     if cluster is not None:
         env["MVO_BA_CLUSTER"] = str(cluster)
     if lib is not None:
         env["MVO_LIB"] = str(lib)
-    code = CHILD.format(root=str(ROOT), tests=str(ROOT / "tests"), py=str(PY), names=list(names))
+    code = CHILD.format(root=str(ROOT), tests=str(ROOT / "tests"), py=str(PY), names=list(names), module=module)
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=timeout, env=env)
     assert r.returncode == 0 and "child ok" in r.stdout, (r.stdout[-1500:], r.stderr[-2500:])
     res = {}
@@ -248,7 +250,7 @@ def run_children(names, cluster=None, lib=None, timeout=1800):
     dbg = {}
     for part in r.stderr.split("@case ")[1:]:
         name, _, rest = part.partition("\n")
-        dbg[name] = parse_debug(rest)
+        dbg[name] = parse(rest)
     return {n: (res[n], dbg.get(n, [])) for n in names}
 
 
