@@ -159,6 +159,19 @@ int mvo_select_uniform_kpts_by_grid(mvo_ctx *ctx, mvo_keypoint *kpts, int *n_kpt
 int mvo_orb_extract_batch_dev(mvo_ctx *ctx, const uint8_t *d_images, int batch, int rows,
                               int cols, int channels, size_t stride, size_t frame_stride,
                               mvo_keypoint *d_kpts, uint8_t *d_desc, int32_t *d_counts, int cap);
+/* geometry::matchFeatures (feature_match.cpp:126-239) for n_pairs frame pairs of a batched extraction, entirely on the
+ * device.  d_kpts / d_desc / d_counts / cap: the layout mvo_orb_extract_batch_dev writes (`batch` frames; counts are
+ * clamped to [0, cap]).  d_pairs: n_pairs x 2 int32 frame indices (query frame, train frame), device memory; any pairs:
+ * consecutive, windowed, reversed, repeated, or a frame with itself.  method_index 1 / 2 / 3 and radius as for
+ * mvo_match_features; method 3 reads the keypoints' pt (d_kpts may be NULL otherwise).
+ * d_out: n_pairs x cap mvo_dmatch, pair p's list at d_out + p * cap, byte-identical to mvo_match_features(query frame,
+ * train frame).  d_n_out[p] = number of matches of pair p, or MVO_ERR_INVALID_ARG (and nothing written to its list) for a
+ * frame index outside [0, batch) or a method-2 pair whose train frame has fewer than 2 keypoints.
+ * cap <= 8192 and n_pairs <= 65535 (MVO_ERR_UNSUPPORTED beyond).  Asynchronous on the context stream: two kernel
+ * launches whatever n_pairs is, no host synchronisation (except when a scratch buffer of the context has to grow). */
+int mvo_match_features_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                                 int batch, int cap, const int32_t *d_pairs, int n_pairs, int method_index, float radius,
+                                 mvo_dmatch *d_out, int32_t *d_n_out);
 
 /* ---- descriptor matching ---------------------------------------------------------------
  * Raw all-pairs kernels.  d1: n1 x 32 bytes (query), d2: n2 x 32 bytes (train).

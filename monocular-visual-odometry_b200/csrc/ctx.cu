@@ -183,7 +183,8 @@ void mvo_destroy(mvo_ctx *ctx) {
   DevBuf *dbs[] = {&ctx->d_a, &ctx->d_b, &ctx->d_c, &ctx->d_d, &ctx->d_e, &ctx->d_f, &ctx->orb_planes,
                    &ctx->orb_cand, &ctx->orb_bandcnt, &ctx->orb_sel, &ctx->orb_misc, &ctx->orb_in,
                    &ctx->orb_kpts, &ctx->orb_desc, &ctx->orb_counts, &ctx->match_part,
-                   &ctx->match_tickets, &ctx->match_in, &ctx->match_keys, &ctx->pnp_pts, &ctx->pnp_hyp,
+                   &ctx->match_tickets, &ctx->match_in, &ctx->match_keys, &ctx->matchb_part, &ctx->matchb_tickets,
+                   &ctx->matchb_keys, &ctx->pnp_pts, &ctx->pnp_hyp,
                    &ctx->pnp_cnt, &ctx->pnp_out, &ctx->ba_buf};
   for (DevBuf *b : dbs)
     if (b->p) cudaFree(b->p);

@@ -17,6 +17,7 @@
 //
 // Arithmetic per pair, Hamming: 8 LOP3 (xor) + 8 LOP3 (carry-save adders) + 4 POPC + 3 adds
 // + 1 pack + 1 min.  No tensor cores: integer/POPC-issue bound (SURVEY.md §8d).
+#include <algorithm>
 #include "mvo_internal.h"
 #include "launch_pdl.cuh"
 
@@ -164,7 +165,167 @@ match_kernel(const uint4 *__restrict__ d1, const float2 *__restrict__ xy1, int n
   }
 }
 
+// The same search over a batch of frame pairs of a batched extraction (mvo_match_features_batch_dev): grid = query tiles x
+// train splits x pairs, sized from the per-frame capacity; both counts are read on the device.  A split covers `span` trains
+// and streams them through shared memory kMaxChunk at a time, so that a batch with many pairs can use one split per tile and
+// skip the merge.  Tiles beyond a pair's query count and splits beyond its train count exit; pairs with a frame index outside
+// [0, batch) (and method-2 pairs with fewer than two trains) are left to the tail kernel, which reports them.
+struct MatchBatchArgs {
+  const uint4 *desc;             // [batch][cap][2]
+  const mvo_keypoint *kpts;      // [batch][cap] (MODE 2: pt)
+  const int32_t *counts;         // [batch]
+  const int2 *pairs;             // [n_pairs] (query frame, train frame)
+  int batch, cap, span;
+  float r2;
+  uint32_t *part;                // [n_pairs][gridDim.y][cap][W] partial winners
+  unsigned int *tickets;         // [n_pairs][gridDim.x], zero between launches
+  uint32_t *keys;                // [n_pairs][cap][W]
+};
+
+template <int MODE>
+__global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
+  pdl_wait();                              // the extraction wrote descriptors, keypoints and counts
+  pdl_launch_dependents();
+  __shared__ uint4 s_t[kMaxChunk * 2];
+  __shared__ float2 s_xy[MODE == 2 ? kMaxChunk : 1];
+  __shared__ bool s_last;
+  const int p = blockIdx.z;
+  const int2 pr = a.pairs[p];
+  if (pr.x < 0 || pr.x >= a.batch || pr.y < 0 || pr.y >= a.batch) return;
+  const int n1 = min(max(a.counts[pr.x], 0), a.cap), n2 = min(max(a.counts[pr.y], 0), a.cap);
+  const int nsplit = (n2 + a.span - 1) / a.span;       // splits that hold trains of this pair
+  const int split = blockIdx.y;
+  if ((int)blockIdx.x * kQ >= n1 || split >= nsplit || (MODE == 1 && n2 < 2)) return;
+  const uint4 *d1 = a.desc + (size_t)pr.x * a.cap * 2, *d2 = a.desc + (size_t)pr.y * a.cap * 2;
+  const mvo_keypoint *k1 = a.kpts + (size_t)pr.x * a.cap, *k2 = a.kpts + (size_t)pr.y * a.cap;
+
+  const int q = blockIdx.x * kQ + threadIdx.x;
+  const int j0 = split * a.span, j1 = min(j0 + a.span, n2);
+  uint32_t qw[8];
+  float qx = 0.f, qy = 0.f;
+  const int qc = min(q, n1 - 1);   // clamp: out-of-range threads compute on a valid row, never store
+  {
+    uint4 u = d1[(size_t)qc * 2], v = d1[(size_t)qc * 2 + 1];
+    qw[0] = u.x; qw[1] = u.y; qw[2] = u.z; qw[3] = u.w;
+    qw[4] = v.x; qw[5] = v.y; qw[6] = v.z; qw[7] = v.w;
+    if (MODE == 2) { qx = k1[qc].x; qy = k1[qc].y; }
+  }
+
+  uint32_t b1 = 0xFFFFFFFFu, b2 = 0xFFFFFFFFu;
+  for (int c0 = j0; c0 < j1; c0 += kMaxChunk) {
+    const int cnt = min(kMaxChunk, j1 - c0);
+    __syncthreads();                       // the previous chunk has been consumed
+    for (int i = threadIdx.x; i < cnt * 2; i += kQ) s_t[i] = d2[(size_t)c0 * 2 + i];
+    if (MODE == 2)
+      for (int i = threadIdx.x; i < cnt; i += kQ) s_xy[i] = make_float2(k2[c0 + i].x, k2[c0 + i].y);
+    __syncthreads();
+#pragma unroll 4
+    for (int j = 0; j < cnt; ++j) {
+      const uint4 t0 = s_t[2 * j], t1 = s_t[2 * j + 1];
+      uint32_t key;
+      if (MODE == 2) {
+        const float2 pt = s_xy[j];
+        const float dx = __fsub_rn(qx, pt.x), dy = __fsub_rn(qy, pt.y);
+        const float dd = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+        const uint32_t d = sad256(qw, t0, t1);
+        key = (dd <= a.r2) ? ((d << 16) | (uint32_t)(c0 + j)) : 0xFFFFFFFFu;
+      } else {
+        key = (hamming256(qw, t0, t1) << 16) | (uint32_t)(c0 + j);
+      }
+      if (MODE == 1) top2_insert(b1, b2, key);
+      else b1 = min(b1, key);
+    }
+  }
+
+  constexpr int W = (MODE == 1) ? 2 : 1;
+  uint32_t *keys = a.keys + (size_t)p * a.cap * W;
+  if (nsplit == 1) {
+    if (q < n1) {
+      keys[(size_t)q * W] = b1;
+      if (MODE == 1) keys[(size_t)q * W + 1] = b2;
+    }
+    return;
+  }
+  uint32_t *part = a.part + (size_t)p * gridDim.y * a.cap * W;
+  if (q < n1) {
+    part[((size_t)split * a.cap + q) * W] = b1;
+    if (MODE == 1) part[((size_t)split * a.cap + q) * W + 1] = b2;
+  }
+  __threadfence();
+  __syncthreads();
+  unsigned int *ticket = a.tickets + (size_t)p * gridDim.x + blockIdx.x;
+  if (threadIdx.x == 0) {
+    unsigned int t = atomicAdd(ticket, 1u);
+    s_last = (t == (unsigned)nsplit - 1);
+    if (s_last) *ticket = 0;               // leave the counter ready for the next launch
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  if (q < n1) {
+    uint32_t m1 = 0xFFFFFFFFu, m2 = 0xFFFFFFFFu;
+    for (int s = 0; s < nsplit; ++s) {
+      const uint32_t *pp = part + ((size_t)s * a.cap + q) * W;
+      const uint32_t x1 = __ldcg(pp);
+      if (MODE == 1) {
+        const uint32_t x2 = __ldcg(pp + 1);
+        top2_insert(m1, m2, x1);
+        top2_insert(m1, m2, x2);
+      } else {
+        m1 = min(m1, x1);
+      }
+    }
+    keys[(size_t)q * W] = m1;
+    if (MODE == 1) keys[(size_t)q * W + 1] = m2;
+  }
+}
+
 }  // namespace
+
+// match_batch_kernel over n_pairs pairs (mvo_internal.h); d_keys: [n_pairs][cap][W] (W = 2 for mode 1)
+int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                           int batch, int cap, const int32_t *d_pairs, int n_pairs, float radius, uint32_t *d_keys) {
+  if (mode < 0 || mode > 2) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "match batch: bad mode %d", mode);
+  if (cap < 1 || cap > 65535 || n_pairs > 65535)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "match batch: cap=%d n_pairs=%d outside [1,65535]", cap, n_pairs);
+  if (n_pairs <= 0) return MVO_OK;
+  const int W = mode == 1 ? 2 : 1;
+  const int qtiles = (cap + kQ - 1) / kQ;
+  // The whole batch, not one pair, has to fill the SMs: about `waves` CTAs per SM over all pairs (the rule of the single-pair
+  // launch above), so a pair gets waves * sm_count / (qtiles * n_pairs) splits, at least one and no shorter than 32 trains.
+  // With a chunk loop in the CTA there is no upper bound on a split's length: 63 pairs of 2001 keypoints run unsplit
+  // (16 tiles x 63 pairs = 1008 CTAs, about 8 per SM on an H100), one pair is split 33 ways as before.
+  const int waves = 4;
+  const long long tiles = (long long)qtiles * n_pairs;
+  int nsplit = (int)std::min<long long>(((long long)waves * ctx->sm_count + tiles - 1) / tiles, 65535);
+  const int max_split = (cap + 31) / 32;
+  if (nsplit > max_split) nsplit = max_split;
+  if (nsplit < 1) nsplit = 1;
+  const int span = (cap + nsplit - 1) / nsplit;
+  nsplit = (cap + span - 1) / span;
+
+  MatchBatchArgs a;
+  a.desc = (const uint4 *)d_desc; a.kpts = d_kpts; a.counts = d_counts; a.pairs = (const int2 *)d_pairs;
+  a.batch = batch; a.cap = cap; a.span = span;
+  a.r2 = radius * radius;   // feature_match.cpp:96
+  a.part = nullptr; a.tickets = nullptr; a.keys = d_keys;
+  if (nsplit > 1) {
+    MVO_TRY(mvo_reserve(ctx, ctx->matchb_part, (size_t)n_pairs * nsplit * cap * W * 4));
+    const size_t had = ctx->matchb_tickets.cap;
+    MVO_TRY(mvo_reserve(ctx, ctx->matchb_tickets, (size_t)n_pairs * qtiles * 4));
+    if (ctx->matchb_tickets.cap != had)    // a new block: zero once, the kernel leaves it zeroed
+      MVO_CUDA(ctx, cudaMemsetAsync(ctx->matchb_tickets.p, 0, ctx->matchb_tickets.cap, ctx->stream));
+    a.part = (uint32_t *)ctx->matchb_part.p;
+    a.tickets = (unsigned int *)ctx->matchb_tickets.p;
+  }
+  dim3 grid(qtiles, nsplit, n_pairs), block(kQ);
+  KTimer kt(ctx, KC_MATCH);
+  if (mode == 0) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<0>, a));
+  else if (mode == 1) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<1>, a));
+  else MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<2>, a));
+  MVO_CHECK_LAUNCH(ctx);
+  return MVO_OK;
+}
 
 int mvo_match_launch(mvo_ctx *ctx, int mode, const uint8_t *d_d1, const float *d_xy1, int n1,
                      const uint8_t *d_d2, const float *d_xy2, int n2, float radius,

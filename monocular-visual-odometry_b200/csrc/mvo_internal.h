@@ -96,6 +96,8 @@ struct mvo_ctx {
   // match
   DevBuf match_part, match_tickets, match_in, match_keys;
   PinBuf match_h;
+  // batched matchFeatures (mvo_match_features_batch_dev): partial winners, merge tickets, packed keys of every pair
+  DevBuf matchb_part, matchb_tickets, matchb_keys;
 
   // timing
   uint32_t timing_mask = 0;
@@ -281,6 +283,10 @@ int mvo_match_launch_masked(mvo_ctx *ctx, int mode, const uint8_t *d_d1, const f
 int mvo_match_launch_ndev(mvo_ctx *ctx, int mode, const uint8_t *d_d1, const float *d_xy1, int n1,
                           const uint8_t *d_d2, const float *d_xy2, int n2, const int32_t *d_n2, float radius,
                           uint32_t *d_keys, const uint8_t *d_qmask);
+// the same over n_pairs frame pairs of a batched extraction (layout of mvo_orb_extract_batch_dev, counts read on the device);
+// d_keys: [n_pairs][cap][W] packed keys, W = 2 for mode 1.  Pairs with an out-of-range frame are skipped
+int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                           int batch, int cap, const int32_t *d_pairs, int n_pairs, float radius, uint32_t *d_keys);
 // pnp.cu: device-resident solvePnPRansac replacement (see there)
 int mvo_pnp_dev_buffers(mvo_ctx *ctx, int n, float **p3, float **p2, double **pose_io, int32_t **out_i, int32_t **inl);
 int mvo_pnp_dev_run(mvo_ctx *ctx, int n, const double *K, const int32_t *d_n);

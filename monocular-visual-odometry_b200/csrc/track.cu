@@ -261,3 +261,41 @@ int mvo_track_match_filter(mvo_ctx *ctx, const MvoTrackFilter &f) {
   ctx->launches++;
   return MVO_OK;
 }
+
+// geometry::matchFeatures over a batch of frame pairs, on the device: match_batch_kernel (match.cu) for all pairs in one launch,
+// then k_match_filter_batch, one CTA per pair.  Two launches whatever n_pairs is; no host synchronisation once the scratch
+// buffers have reached their size.
+extern "C" int mvo_match_features_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                                            int batch, int cap, const int32_t *d_pairs, int n_pairs, int method_index, float radius,
+                                            mvo_dmatch *d_out, int32_t *d_n_out) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (method_index < 1 || method_index > 3)   // feature_match.cpp:225 throws
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "matchFeatures batch: wrong method index %d", method_index);
+  if (n_pairs < 0 || batch < 1 || cap < 1)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "matchFeatures batch: n_pairs=%d batch=%d cap=%d", n_pairs, batch, cap);
+  if (!d_desc || !d_counts || !d_pairs || !d_out || !d_n_out || (method_index == 3 && !d_kpts))
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "matchFeatures batch: null pointer");
+  if (cap > MF_MAXN) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "matchFeatures batch: cap %d above the device filter's %d", cap, MF_MAXN);
+  if (n_pairs > 65535) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "matchFeatures batch: %d pairs, at most 65535 per call", n_pairs);
+  if (n_pairs == 0) return MVO_OK;
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int mode = method_index == 1 ? 0 : (method_index == 2 ? 1 : 2);
+  const int W = mode == 1 ? 2 : 1;
+  MVO_TRY(mvo_reserve(ctx, ctx->matchb_keys, (size_t)n_pairs * cap * W * 4));
+  uint32_t *keys = (uint32_t *)ctx->matchb_keys.p;
+  MVO_TRY(mvo_match_batch_launch(ctx, mode, d_kpts, d_desc, d_counts, batch, cap, d_pairs, n_pairs, radius, keys));
+
+  int n_cap = 2048;
+  while (n_cap < cap) n_cap *= 2;
+  FilterBatchArgs b;
+  b.keys = keys; b.counts = d_counts; b.pairs = (const int2 *)d_pairs;
+  b.batch = batch; b.cap = cap; b.method = method_index; b.n_cap = n_cap;
+  b.xg_ratio = ctx->prm.xiang_gao_ratio; b.lowe_ratio = ctx->prm.lowe_ratio;
+  b.out = d_out; b.n_out = d_n_out;
+  const size_t smem = (size_t)n_cap * (4 + 4 + 2 + 2 + 2) + 3 * ((size_t)n_cap / 16 + 2) * 4 + ((size_t)n_cap / 16 + 2) + 64;
+  MVO_CUDA(ctx, cudaFuncSetAttribute(k_match_filter_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  KTimer kt(ctx, KC_MATCH);
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)n_pairs, MF_T, smem, 0, k_match_filter_batch, b));
+  ctx->launches++;
+  return MVO_OK;
+}

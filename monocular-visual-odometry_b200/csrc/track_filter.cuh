@@ -1,5 +1,6 @@
-// The match-list filter kernel (k_match_filter: thresholds of matchFeatures + removeDuplicatedMatches restated on the device,
-// see the comment in track.cu) and the projection helper it shares with the other tracking kernels — the text nvcc
+// The match-list filter kernels (k_match_filter: thresholds of matchFeatures + removeDuplicatedMatches restated on the device,
+// see the comment in track.cu; k_match_filter_batch: the same body once per frame pair of mvo_match_features_batch_dev) and the
+// projection helper they share with the other tracking kernels — the text nvcc
 // compiles, in a header so that the CPU test tier can build it for the host (tests/cpp/track_filter_emu.cpp, through
 // tests/cpp/cuda_emu.h).  Included by track.cu inside an anonymous namespace.
 // MVO_DYN_SMEM(type, name) declares the kernel's dynamic shared memory (`extern __shared__ __align__(16) type name[]` for nvcc).
@@ -168,8 +169,10 @@ __device__ __forceinline__ int mf_partition_warp(uint32_t *arr, uint16_t *Ls, ui
   return cut;
 }
 
-__global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
-  MVO_DYN_SMEM(uint8_t, smraw);
+// The body of the filter, run by one CTA of MF_T threads over one match list.  kAllVisible: every query takes part (a.vis and
+// a.project are not read; the batched matchFeatures tail).  emit(o, query, train) writes the o-th surviving pair.
+template <bool kAllVisible, class Emit>
+__device__ __forceinline__ void match_filter_run(const FilterArgs &a, uint8_t *smraw, Emit emit) {
   const int cap = a.n_cap;
   uint32_t *arr = (uint32_t *)smraw;                    // [cap]  (train << 16) | position in the match list
   uint32_t *best = arr + cap;                           // [cap]  per keypoint: leftmost (position << 16 | list index)
@@ -196,7 +199,8 @@ __global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
   __syncthreads();
   // ---- thresholds (feature_match.cpp:179-196 for methods 1/3, :210-217 for method 2), ordered compaction ----
   const int per = (nmap + MF_T - 1) / MF_T, q0 = min(tid * per, nmap), q1 = min(q0 + per, nmap);
-  if (a.project) {          // every thread reads back only the flags it wrote itself
+  auto visible = [&](int q) -> bool { return kAllVisible || a.vis[q] != 0; };
+  if (!kAllVisible && a.project) {          // every thread reads back only the flags it wrote itself
     Rt12 Tcw = a.Tcw;
     if (a.d_Tcw) {          // enqueued ahead of time: the reference keyframe's pose as the bundle adjustment of the previous frame left it
 #pragma unroll
@@ -208,7 +212,7 @@ __global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
   if (a.method != 2) {
     unsigned m = 0xFFFFFFFFu;
     for (int q = q0; q < q1; ++q) {
-      if (!a.vis[q]) continue;
+      if (!visible(q)) continue;
       ++nvis;
       const uint32_t k = a.keys[q];
       if (k != 0xFFFFFFFFu) m = min(m, k >> 16);
@@ -217,7 +221,7 @@ __global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
     for (int o = 16; o > 0; o >>= 1) m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (lane == 0 && m != 0xFFFFFFFFu) atomicMin(&s_min, m);
   } else {
-    for (int q = q0; q < q1; ++q) nvis += a.vis[q] != 0;
+    for (int q = q0; q < q1; ++q) nvis += visible(q);
   }
   __syncthreads();
   double thr = 0;
@@ -227,7 +231,7 @@ __global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
     thr = (double)fmaxf((float)(min_dis * a.xg_ratio), 30.0f);        // std::max<float>(min_dis * ratio, 30.0)
   }
   auto passes = [&](int q, uint32_t &train) -> bool {
-    if (!a.vis[q]) return false;
+    if (!visible(q)) return false;
     if (a.method != 2) {
       const uint32_t k = a.keys[q];
       if (k == 0xFFFFFFFFu) return false;
@@ -356,16 +360,81 @@ __global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
   int o = block_excl_scan(c2, s_warp, np);
   for (int t = t0; t < t1; ++t)
     if (best[t] != 0xFFFFFFFFu) {
-      const int mi = (int)amap[best[t] & 0xFFFFu];
-      a.pairs[o] = make_int2(mi, t);
-      if (a.p3) {
-        a.p3[3 * o] = a.map_pts[3 * mi]; a.p3[3 * o + 1] = a.map_pts[3 * mi + 1]; a.p3[3 * o + 2] = a.map_pts[3 * mi + 2];
-        a.p2[2 * o] = a.kpts[t].x; a.p2[2 * o + 1] = a.kpts[t].y;
-      }
+      emit(o, (int)amap[best[t] & 0xFFFFu], t);
       ++o;
     }
   if (tid == 0) { a.info[0] = np; a.info[1] = ncand; a.info[2] = 0; }
   MF_MARK(2);
 #undef MF_MARK
+}
+
+// The tracker's filter: map points (queries) in view of the guess pose against the frame's keypoints (trains); the pairs and,
+// optionally, the PnP input arrays
+__global__ void __launch_bounds__(MF_T, 1) k_match_filter(FilterArgs a) {
+  MVO_DYN_SMEM(uint8_t, smraw);
+  match_filter_run<false>(a, smraw, [&](int o, int mi, int t) {
+    a.pairs[o] = make_int2(mi, t);
+    if (a.p3) {
+      a.p3[3 * o] = a.map_pts[3 * mi]; a.p3[3 * o + 1] = a.map_pts[3 * mi + 1]; a.p3[3 * o + 2] = a.map_pts[3 * mi + 2];
+      a.p2[2 * o] = a.kpts[t].x; a.p2[2 * o + 1] = a.kpts[t].y;
+    }
+  });
+}
+
+// The tail of geometry::matchFeatures for a batch of frame pairs (mvo_match_features_batch_dev): one CTA per pair over the packed
+// keys of match_batch_kernel (match.cu), every query visible, the surviving matches written as cv::DMatch records.  Per pair:
+// n_out[p] = number of matches, or MVO_ERR_INVALID_ARG (no writes to out) for a frame index outside [0, batch) or a method-2 pair
+// whose train frame has fewer than 2 keypoints.
+struct FilterBatchArgs {
+  const uint32_t *keys;     // [n_pairs][cap][W]
+  const int32_t *counts;    // [batch]
+  const int2 *pairs;        // [n_pairs] (query frame, train frame)
+  int batch, cap, method, n_cap;
+  double xg_ratio, lowe_ratio;
+  mvo_dmatch *out;          // [n_pairs][cap]
+  int32_t *n_out;           // [n_pairs]
+};
+
+__global__ void __launch_bounds__(MF_T, 1) k_match_filter_batch(FilterBatchArgs b) {
+  MVO_DYN_SMEM(uint8_t, smraw);
+  __shared__ int32_t s_info[24];
+  // match_filter_run waits again: griddepcontrol.wait returns at once when the predecessor has already been waited for
+  pdl_wait();
+  pdl_launch_dependents();
+  const int p = blockIdx.x;
+  const int2 pr = b.pairs[p];
+  const int W = b.method == 2 ? 2 : 1;
+  if (pr.x < 0 || pr.x >= b.batch || pr.y < 0 || pr.y >= b.batch) {
+    if (threadIdx.x == 0) b.n_out[p] = MVO_ERR_INVALID_ARG;
+    return;
+  }
+  const int n1 = min(max(b.counts[pr.x], 0), b.cap), n2 = min(max(b.counts[pr.y], 0), b.cap);
+  if (b.method == 2 && n2 < 2) {            // knnMatch(k = 2) needs two trains: mvo_match_features fails there
+    if (threadIdx.x == 0) b.n_out[p] = MVO_ERR_INVALID_ARG;
+    return;
+  }
+  if (n1 == 0 || n2 == 0) {                 // no query, or BFMatcher / the radius search over an empty train set: no matches
+    if (threadIdx.x == 0) b.n_out[p] = 0;
+    return;
+  }
+  FilterArgs a = {};
+  a.keys = b.keys + (size_t)p * b.cap * W;
+  a.nmap = n1; a.nk = n2; a.method = b.method; a.n_cap = b.n_cap;
+  a.xg_ratio = b.xg_ratio; a.lowe_ratio = b.lowe_ratio;
+  a.info = s_info;
+  const uint32_t *keys = a.keys;
+  mvo_dmatch *out = b.out + (size_t)p * b.cap;
+  const int method = b.method;
+  match_filter_run<true>(a, smraw, [&](int o, int qi, int t) {
+    // unpack() of match_host.cpp: the best key of the query; method 3's distance is the SAD / 32 through double, img_idx -1
+    const uint32_t d = keys[(size_t)qi * W] >> 16;
+    mvo_dmatch m;
+    m.query_idx = qi;
+    m.train_idx = t;
+    m.img_idx = method == 3 ? -1 : 0;
+    m.distance = method == 3 ? (float)((double)d / 32.0) : (float)d;
+    out[o] = m;
+  });
+  if (threadIdx.x == 0) b.n_out[p] = s_info[2] == 0 ? s_info[0] : MVO_ERR_UNSUPPORTED;   // s_info: written by this thread
 }
 

@@ -102,6 +102,7 @@ SIGNATURES = {
     "mvo_orb_extract": (_i, [_vp, _vp, _i, _i, _i, _sz, _vp, _pi, _vp]),
     "mvo_select_uniform_kpts_by_grid": (_i, [_vp, _vp, _pi, _i, _i]),
     "mvo_orb_extract_batch_dev": (_i, [_vp, _vp, _i, _i, _i, _i, _sz, _sz, _vp, _vp, _vp, _i]),
+    "mvo_match_features_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _f, _vp, _vp]),
     "mvo_match_hamming_nn": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "mvo_match_hamming_knn2": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "mvo_match_radius_sad": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _f, _vp, _pi]),
@@ -298,6 +299,12 @@ class Context:
     def orb_extract_batch_dev(self, d_images, batch, rows, cols, ch, stride, frame_stride, d_kpts, d_desc, d_counts, cap):
         self._chk(self.lib.mvo_orb_extract_batch_dev(self.h, _ptr(d_images), batch, rows, cols, ch, stride,
                                                      frame_stride, _ptr(d_kpts), _ptr(d_desc), _ptr(d_counts), cap))
+
+    def match_features_batch_dev(self, d_kpts, d_desc, d_counts, batch, cap, d_pairs, n_pairs, method_index, radius, d_out, d_n_out):
+        """matchFeatures for n_pairs (query frame, train frame) pairs of an orb_extract_batch_dev output, all device pointers;
+        pair p's matches land at d_out + p * cap records, their count (or MVO_ERR_INVALID_ARG for a bad pair) in d_n_out[p]."""
+        self._chk(self.lib.mvo_match_features_batch_dev(self.h, _ptr(d_kpts), _ptr(d_desc), _ptr(d_counts), batch, cap, _ptr(d_pairs),
+                                                        n_pairs, method_index, C.c_float(radius), _ptr(d_out), _ptr(d_n_out)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):
