@@ -153,10 +153,11 @@ k_pyramid(OrbPlanDev plan, const uint8_t *__restrict__ in, int channels, size_t 
     const int lo = bt[0], hi = bt[1], olo = bt[2], ohi = bt[3], wpr = L.pitch >> 2;
     const uint8_t *base = in + (size_t)f * frame_stride;
     const bool aligned = ((reinterpret_cast<uintptr_t>(base) | stride) & 3) == 0;
+    const bool keep = nl > 1;                                      // a single level is not a source: no shared memory is sized for it
     for (int i = tid; i < (hi - lo) * wpr; i += PYR_T) {
       const int r = i / wpr, x4 = (i - r * wpr) << 2, y = lo + r;
       const uint32_t v = gray4(base + (size_t)y * stride, x4, L.w, channels, aligned);
-      *reinterpret_cast<uint32_t *>(s_prev + (size_t)r * L.pitch + x4) = v;
+      if (keep) *reinterpret_cast<uint32_t *>(s_prev + (size_t)r * L.pitch + x4) = v;
       if (y >= olo && y < ohi) *reinterpret_cast<uint32_t *>(slot + L.img_off + (size_t)y * L.pitch + x4) = v;
     }
   }
@@ -462,6 +463,12 @@ k_fast(OrbPlanDev plan, const uint8_t *__restrict__ planes, uint32_t *__restrict
   }
 }
 
+// Cell of a keypoint in the uncovered strip right of column grid_cols * grid_size or below row grid_rows * grid_size (images whose
+// size is not a multiple of the grid size).  The reference indexes its grid out of range there (feature_match.cpp:70-72, undefined
+// behaviour); the project's reading is that such a keypoint is skipped: it is not kept and uses up no cell's quota.  The host
+// selection (orb_host.cpp: grid_select) and the oracle do the same, so a frame selects the same keypoints on every path.
+constexpr int ORB_NO_CELL = 0xFFFF;      // grid_rows * grid_cols <= 65535: never a real cell
+
 // cell index = (int)coordinate / grid_size (feature_match.cpp:70): a shift when the grid size is a power of two (the coordinates are >= 0)
 __device__ __forceinline__ int orb_grid_shift(int g) {
   if (g <= 0 || (g & (g - 1)) != 0) return -1;
@@ -491,6 +498,7 @@ __device__ __forceinline__ void grid_rank_keep(int n, const uint16_t *__restrict
     for (int i = tid; i < n; i += 1024) {
       if (s_keep[i]) continue;
       const int c = s_cell[i];
+      if (c == ORB_NO_CELL) continue;
       if (r > 0 && prev[c] == (tag_prev | (uint32_t)i)) { s_keep[i] = 1; continue; }
       if (r < max_per_cell) atomicMin(&cur[c], tag | (uint32_t)i);
     }
@@ -516,8 +524,8 @@ __device__ __forceinline__ void grid_rank_keep_seg(int n, const uint16_t *__rest
   const unsigned lt = lanemask_lt();
   for (int i0 = b; i0 < e; i0 += 32) {
     const int i = i0 + lane;
-    const bool in = i < e;
-    const unsigned c = in ? (unsigned)s_cell[i] : 0xFFFF0000u + (unsigned)lane;      // lanes past the end: a group of their own
+    const bool in = i < e && s_cell[i] != ORB_NO_CELL;
+    const unsigned c = in ? (unsigned)s_cell[i] : 0xFFFF0000u + (unsigned)lane;      // lanes past the end or outside the grid: a group of their own
     const unsigned peers = __match_any_sync(0xffffffffu, c);
     const int leader = 31 - __clz((int)peers);               // only the group's highest lane touches the count: one warp barrier per step
     int base = 0;
@@ -542,7 +550,10 @@ __device__ __forceinline__ void grid_rank_keep_seg(int n, const uint16_t *__rest
   __syncthreads();
   for (int i0 = b; i0 < e; i0 += 32) {
     const int i = i0 + lane;
-    if (i < e) s_keep[i] = (uint8_t)(((int)s_keep[i] + (int)tab[s_cell[i]]) < max_per_cell);
+    if (i < e) {
+      const int c = s_cell[i];
+      s_keep[i] = (uint8_t)(c != ORB_NO_CELL && ((int)s_keep[i] + (int)tab[c]) < max_per_cell);
+    }
   }
   __syncthreads();
 }
@@ -629,10 +640,7 @@ k_select(OrbPlanDev plan, const uint32_t *__restrict__ staging, const int32_t *_
           const float fx = l ? __fmul_rn((float)orb_px(p), scale) : (float)orb_px(p);
           const float fy = l ? __fmul_rn((float)orb_py(p), scale) : (float)orb_py(p);
           int row = gshift >= 0 ? ((int)fy) >> gshift : ((int)fy) / plan.grid_size, col = gshift >= 0 ? ((int)fx) >> gshift : ((int)fx) / plan.grid_size;
-          row = min(row, plan.grid_rows - 1);
-          col = min(col, plan.grid_cols - 1);
-          const int cell = row * plan.grid_cols + col;
-          s_cell[o + i] = (uint16_t)cell;
+          s_cell[o + i] = (uint16_t)(row < plan.grid_rows && col < plan.grid_cols ? row * plan.grid_cols + col : ORB_NO_CELL);
         }
       }
     }
@@ -981,10 +989,8 @@ k_select_kept(OrbPlanDev plan, const uint32_t *__restrict__ cand, const uint16_t
       const float fx = l ? __fmul_rn((float)orb_px(p), scale) : (float)orb_px(p);
       const float fy = l ? __fmul_rn((float)orb_py(p), scale) : (float)orb_py(p);
       int row = gshift >= 0 ? ((int)fy) >> gshift : ((int)fy) / plan.grid_size, col = gshift >= 0 ? ((int)fx) >> gshift : ((int)fx) / plan.grid_size;
-      row = min(row, plan.grid_rows - 1);
-      col = min(col, plan.grid_cols - 1);
-      const int cell = row * plan.grid_cols + col;
-      s_pk[i] = p; s_lvl[i] = (uint8_t)l; s_cell[i] = (uint16_t)cell;
+      s_pk[i] = p; s_lvl[i] = (uint8_t)l;
+      s_cell[i] = (uint16_t)(row < plan.grid_rows && col < plan.grid_cols ? row * plan.grid_cols + col : ORB_NO_CELL);
     }
   }
   __syncthreads();
@@ -1266,7 +1272,7 @@ k_test_grid_rank(const uint16_t *__restrict__ cells, int n, int ncell, int max_p
 
 }  // namespace
 
-// test hook (not part of mvo.h): cells[i] < ncell, n <= 16384; seg = 1: grid_rank_keep_seg, 0: grid_rank_keep (rounds)
+// test hook (not part of mvo.h): cells[i] < ncell or 0xFFFF (outside the grid: never kept), n <= 16384; seg = 1: grid_rank_keep_seg, 0: grid_rank_keep (rounds)
 extern "C" int mvo_test_grid_rank(mvo_ctx *ctx, const uint16_t *cells, int n, int ncell, int max_per_cell, int seg, uint8_t *keep) {
   if (!ctx || !cells || !keep || n < 1 || n > 16384 || ncell < 1 || ncell > 4096 || max_per_cell < 0) return MVO_ERR_INVALID_ARG;
   if (seg && max_per_cell > 254) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "grid_rank_keep_seg: per-cell limit above the byte counters");

@@ -38,6 +38,7 @@ void axis_table(int src, int dst, int32_t *ofs, int32_t *w1) {
 
 int build_plan(mvo_ctx *ctx, OrbState *st, int rows, int cols) {
   const mvo_params &P = ctx->prm;
+  st->valid = false;           // a plan rejected below must not be taken for the previous one by the next call (ensure_ws)
   if (rows < 2 * ORB_EDGE + 8 || cols < 2 * ORB_EDGE + 8)
     return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "image %dx%d too small for ORB (edge threshold 31)", cols, rows);
   if (cols >= ORB_MAX_W || rows >= ORB_MAX_W)
@@ -79,8 +80,9 @@ int build_plan(mvo_ctx *ctx, OrbState *st, int rows, int cols) {
   for (int l = 0; l < pl.nlevels; ++l) {
     OrbLevelDev &L = pl.lv[l];
     L.scale = (float)pow(scale_factor, (double)l);
-    L.w = cv_round((double)((float)cols / L.scale));
-    L.h = cv_round((double)((float)rows / L.scale));
+    const float inv = 1.0f / L.scale;                            // OpenCV orb.cpp: Size(cvRound(cols * invScale), cvRound(rows * invScale))
+    L.w = cv_round((double)((float)cols * inv));                 // (cols / scale rounds the other way for e.g. 153 rows: 128 vs 127)
+    L.h = cv_round((double)((float)rows * inv));
     if (L.w < 2 * ORB_EDGE + 2 || L.h < 2 * ORB_EDGE + 2) break;    // level has no pixel inside the border
     L.pitch = (L.w + 127) & ~127;
     L.img_off = (uint32_t)off;
@@ -235,7 +237,7 @@ std::vector<int> grid_select(int n, GetXY xy, int rows, int cols, int grid, int 
     float x, y;
     xy(i, x, y);
     int row = ((int)y) / grid, col = ((int)x) / grid;
-    if (row < 0 || col < 0 || row >= gr || col >= gc) continue;   // reference indexes out of bounds here (UB)
+    if (row < 0 || col < 0 || row >= gr || col >= gc) continue;   // reference indexes out of bounds here (UB): skipped, as k_select does
     if (cnt[(size_t)row * gc + col] < max_per_cell) {
       keep.push_back(i);
       cnt[(size_t)row * gc + col]++;

@@ -158,7 +158,9 @@ int orc_select_uniform_kpts_by_grid(OrcKeyPoint *kp, int n, int image_rows, int 
   for (int i = 0; i < n; ++i) {
     const OrcKeyPoint &kpt = kp[i];
     int row = ((int)kpt.y) / grid_size, col = ((int)kpt.x) / grid_size;
-    if (row < 0 || row >= rows || col < 0 || col >= cols) continue;  // reference: out-of-bounds UB; never hit for ORB output
+    // reference: out-of-bounds UB for a keypoint in the strip right of / below the last whole cell (image size not a multiple of
+    // grid_size, strip wider than the 31-px ORB border); the project's reading, shared by the library's device and host paths: skipped
+    if (row < 0 || row >= rows || col < 0 || col >= cols) continue;
     if (grid[row][col] < max_pts_per_grid) {
       tmp.push_back(kpt);
       grid[row][col]++;

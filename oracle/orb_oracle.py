@@ -56,8 +56,8 @@ def _cv_round(x):
 def level_sizes(cols, rows, nlevels, scale_factor):
     out = []
     for s in level_scales(nlevels, scale_factor):
-        inv = np.float32(1.0) / s     # Size(cvRound(cols/scale)) with float scale
-        out.append((_cv_round(np.float32(cols) / s), _cv_round(np.float32(rows) / s)))
+        inv = np.float32(1.0) / s     # Size(cvRound(cols * invScale), cvRound(rows * invScale)), float invScale = 1.0f / scale
+        out.append((_cv_round(np.float32(np.float32(cols) * inv)), _cv_round(np.float32(np.float32(rows) * inv))))
     return out
 
 

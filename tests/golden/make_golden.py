@@ -51,6 +51,28 @@ def make_orb():
                             cv_version=cv2.__version__, **extra)
 
 
+# small cases of tests/orb_cases.py at non-default parameters: one level, three at 1.5, eight at 1.2, both sides of the packed /
+# scalar FAST threshold switch, the highest threshold, and a 64-px grid with keypoints in the uncovered strip on the retainBest path
+ORB_PARAM_GOLDENS = ["nl1_200x152", "nl3_sf1.5_203x161", "nl8_sf1.2_256x240", "t127_dots", "t128_dots", "t254_dots",
+                     "grid64_strip_250x200_retain"]
+
+
+def make_orb_params():
+    """cv::ORB at the parameters of ORB_PARAM_GOLDENS -> selectUniformKptsByGrid restatement -> compute: orb_params.npz holds
+    <case>/image, /selected, /descriptors and /counts (FAST candidates inside the border per level)."""
+    import cv2
+    sys.path.insert(0, str(ROOT / "tests"))
+    import orb_cases as O
+    out = {}
+    for name in ORB_PARAM_GOLDENS:
+        c = O.CASE[name]
+        img = O.image(c)
+        sel, desc, counts = O.reference_cv2(img, c["p"])
+        out.update({f"{name}/image": img, f"{name}/selected": sel, f"{name}/descriptors": desc,
+                    f"{name}/counts": np.array(counts, np.int32)})
+    np.savez_compressed(OUT / "orb_params.npz", cv_version=cv2.__version__, **out)
+
+
 def make_pnp():
     """cv::solvePnPRansac exactly as called at src/vo/vo.cpp:318-320 on the config-3 instance."""
     import cv2
@@ -72,5 +94,7 @@ if __name__ == "__main__":
         make_match()
     if what in ("orb", "all") and "make_orb" in globals():
         make_orb()
+    if what in ("orb", "all"):
+        make_orb_params()
     if what in ("pnp", "all") and "make_pnp" in globals():
         make_pnp()
