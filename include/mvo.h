@@ -172,6 +172,36 @@ int mvo_orb_extract_batch_dev(mvo_ctx *ctx, const uint8_t *d_images, int batch, 
 int mvo_match_features_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
                                  int batch, int cap, const int32_t *d_pairs, int n_pairs, int method_index, float radius,
                                  mvo_dmatch *d_out, int32_t *d_n_out);
+/* geometry::estiMotionByEssential (+ doTriangulation) for the matched frame pairs of a batch, entirely on the device: what
+ * mvo_estimate_relative_poses(calc_homo = 0, motion_cam2_to_cam1 = 1) returns as its solution 0, pair by pair.
+ * d_kpts / d_counts / batch / cap: the layout of mvo_orb_extract_batch_dev (counts clamped to [0, cap]).  d_pairs: n_pairs x 2
+ * int32 (query frame, train frame); d_matches / d_n_matches: what mvo_match_features_batch_dev wrote for those pairs (pair p's
+ * list at d_matches + p * cap).  Pair p's correspondences are pts1[i] = kpts[query frame][m_i.query_idx].pt and pts2[i] =
+ * kpts[train frame][m_i.train_idx].pt in match-list order; K: host 3x3, threshold: pixels (mvo_params::essential_threshold of the
+ * per-pair path).  Every pair uses mvo_params::epi_hypotheses and pnp_seed as a single call on its points does.
+ * d_res[p]: status MVO_OK, or the mvo_status of that pair alone; then nothing else of the pair is written (not the rest of
+ * its record, its inlier rows or its points):
+ *   MVO_ERR_INVALID_ARG  a frame index outside [0, batch), a match count outside [0, cap], a query_idx / train_idx outside
+ *                        [0, count) of its frame (checked before anything is read through it);
+ *   MVO_ERR_DEGENERATE   fewer than 8 matches, or no model reaches 8 inliers.
+ * On MVO_OK: E, R, t byte-identical to mvo_esti_motion_by_essential on those points; d_inliers + p * cap: the n_inliers
+ * inlier indices into the pair's match list, ascending; d_pts3d (NULL: no triangulation) + p * cap * 3: the inliers
+ * triangulated as mvo_do_triangulation does on pixel2CamNormPlane points.
+ * MVO_ERR_INVALID_ARG: a null pointer, fx or fy <= 0, threshold <= 0.  MVO_ERR_UNSUPPORTED: cap > 6400 (the consensus
+ * kernel's shared memory, as for a single call), n_pairs > 65535, n_pairs x epi_hypotheses > 2^22 (80 bytes of scratch per
+ * hypothesis).  Asynchronous on the context stream: six kernel launches (seven with d_pts3d) whatever n_pairs is, no host
+ * synchronisation except when the call's own scratch buffer of the context has to grow. */
+typedef struct mvo_two_view_result {
+  int32_t status;      /* MVO_OK, or the mvo_status the per-pair call would have returned */
+  int32_t n_matches;   /* correspondences of the pair (its match count) */
+  int32_t n_inliers;   /* findEssentialMat's mask count; rows of the pair's inlier list */
+  int32_t votes;       /* recoverPose's good-point count of the chosen (R, t) */
+  double E[9], R[9], t[3];   /* as mvo_esti_motion_by_essential returns them: E[8] = 1, x2 ~ R x1 + t, |t| = 1 */
+} mvo_two_view_result;
+int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                           const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
+                                           const int32_t *d_n_matches, const double *K, double threshold,
+                                           mvo_two_view_result *d_res, int32_t *d_inliers, float *d_pts3d);
 
 /* ---- descriptor matching ---------------------------------------------------------------
  * Raw all-pairs kernels.  d1: n1 x 32 bytes (query), d2: n2 x 32 bytes (train).

@@ -14,6 +14,8 @@
 //   k_epi_score       one warp per hypothesis, points staged once per CTA in shared memory, count(Sampson <= thr^2)
 //   k_epi_finish      one CTA: arg-max (ties -> lowest hypothesis), ordered inlier list, recoverPose vote
 //   k_triangulate     one thread per point: epi::triangulate_dlt
+// mvo_esti_motion_by_essential_batch_dev runs the same kernel bodies over a batch of matched frame pairs (a pair dimension on
+// every kernel, one finish cluster per pair, recoverPose's pick on the device: epipolar_kernels.cuh, "batch of frame pairs").
 // The numerics live in epipolar_math.cuh and are unit-tested on the host (tests/test_epipolar_math.py).
 #include <cooperative_groups.h>
 #include <stdlib.h>
@@ -72,13 +74,14 @@ __global__ void k_epi_math_test(const double *__restrict__ in, double *__restric
   for (int q = 0; q < 3; ++q) out[61 + q] = w2[q];
 }
 
-// one thread-block cluster of EFIN_C CTAs (distributed shared memory between them), all block state in dynamic shared memory
+// `clusters` thread-block clusters of EFIN_C CTAs each (distributed shared memory between them), one after the other along x;
+// all block state in dynamic shared memory
 template <class K, class... A>
-cudaError_t launch_finish_cluster(mvo_ctx *ctx, size_t smem, K kernel, A... args) {
+cudaError_t launch_finish_cluster(mvo_ctx *ctx, unsigned clusters, size_t smem, K kernel, A... args) {
   static const int env_c = getenv("MVO_EFIN_CLUSTER") ? atoi(getenv("MVO_EFIN_CLUSTER")) : EFIN_C;     // A/B hook: CTAs per cluster
   const int csz = (env_c >= 1 && env_c <= 8) ? env_c : EFIN_C;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(csz);
+  cfg.gridDim = dim3(csz * clusters);
   cfg.blockDim = dim3(EFIN_T);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = ctx->stream;
@@ -130,6 +133,73 @@ int mvo_epi_essential_ex(mvo_ctx *ctx, const float *pts1, const float *pts2, int
   MvoEpiJob job;
   MVO_TRY(mvo_epi_essential_begin(ctx, pts1, pts2, n, K, threshold, want_pose, tri_np1, tri_np2, tri_R, tri_t, tri_out != nullptr, &job));
   return mvo_epi_essential_end(ctx, &job, E, R, t, inliers, n_inliers, tri_out);
+}
+
+// mvo_esti_motion_by_essential_batch_dev (mvo.h): gather, hypotheses, scoring, finish, vote, pick (+ triangulation) for every
+// pair at once; the scratch lives in ctx->epib_buf
+extern "C" int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                                      const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
+                                                      const int32_t *d_n_matches, const double *K, double threshold,
+                                                      mvo_two_view_result *d_res, int32_t *d_inliers, float *d_pts3d) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (!d_kpts || !d_counts || !d_pairs || !d_matches || !d_n_matches || !K || !d_res || !d_inliers)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: null pointer");
+  if (n_pairs < 0 || batch < 1 || cap < 1)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: n_pairs=%d batch=%d cap=%d", n_pairs, batch, cap);
+  if (!(K[0] > 0 && K[4] > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal lengths must be positive");
+  if (!(threshold > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: threshold must be positive");
+  const size_t smem = (size_t)cap * 4 * sizeof(double);
+  if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential batch: cap %d above %d correspondences", cap, 200 * 1024 / 32);
+  if (n_pairs > 65535) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential batch: %d pairs, at most 65535 per call", n_pairs);
+  const int H = ctx->prm.epi_hypotheses;
+  if ((size_t)n_pairs * H > ((size_t)1 << 22))
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential batch: %d pairs x %d hypotheses above 2^22 per call", n_pairs, H);
+  if (n_pairs == 0) return MVO_OK;
+  EpiCam cam;
+  cam.f = (K[0] + K[4]) / 2; cam.cx = K[2]; cam.cy = K[5];
+  const bool tri = d_pts3d != nullptr;
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t np = (size_t)n_pairs, pts = al(np * cap * 8);
+  const size_t o_p1 = 0, o_p2 = o_p1 + pts, o_n1 = o_p2 + pts, o_n2 = o_n1 + (tri ? pts : 0), o_pn = o_n2 + (tri ? pts : 0);
+  const size_t o_E = al(o_pn + np * 4), o_valid = al(o_E + np * H * 72), o_cnt = al(o_valid + np * H * 4), o_od = al(o_cnt + np * H * 4);
+  const size_t o_oi = al(o_od + np * EPIB_OUT_D * 8), o_end = o_oi + np * EPIB_OUT_I * 4;
+  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, o_end));
+  uint8_t *d = (uint8_t *)ctx->epib_buf.p;
+  float *p1 = (float *)(d + o_p1), *p2 = (float *)(d + o_p2), *np1 = tri ? (float *)(d + o_n1) : nullptr, *np2 = tri ? (float *)(d + o_n2) : nullptr;
+  int32_t *pn = (int32_t *)(d + o_pn), *valid = (int32_t *)(d + o_valid), *cnt = (int32_t *)(d + o_cnt), *oi = (int32_t *)(d + o_oi);
+  double *Es = (double *)(d + o_E), *od = (double *)(d + o_od);
+  const double thr2 = (threshold / cam.f) * (threshold / cam.f);          // as mvo_epi_essential_begin
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_gather<<<n_pairs, 256, 0, ctx->stream>>>(d_kpts, d_counts, batch, cap, (const int2 *)d_pairs, d_matches, d_n_matches, K[0], K[4], K[2], K[5],
+                                                 p1, p2, np1, np2, pn); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_hypotheses_batch<<<dim3((H + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(p1, p2, pn, cap, cam, ctx->prm.pnp_seed, H, Es, valid); }
+  MVO_CHECK_LAUNCH(ctx);
+  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_epi_score_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // about as many CTAs in all as the single call uses for its one pair, at least one per pair
+  int per_pair = (4 * ctx->sm_count + n_pairs - 1) / n_pairs;
+  if (per_pair > (H + 7) / 8) per_pair = (H + 7) / 8;
+  { KTimer kt(ctx, KC_EPI_SCORE);
+  k_epi_score_batch<<<dim3(per_pair, n_pairs), 256, smem, ctx->stream>>>(p1, p2, pn, cap, cam, thr2, H, Es, valid, cnt); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI_FINISH);
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(EpiFinSmem), k_epi_finish_batch, (const float *)p1, (const float *)p2,
+                                        (const int32_t *)pn, cap, cam, thr2, H, (const double *)Es, (const int32_t *)cnt, od, oi, d_inliers)); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_vote_batch<<<dim3((cap + 63) / 64, n_pairs), 256, 0, ctx->stream>>>(p1, p2, pn, cap, cam, od, oi, d_inliers); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_pick<<<(n_pairs + 127) / 128, 128, 0, ctx->stream>>>(pn, n_pairs, od, oi, d_res); }
+  MVO_CHECK_LAUNCH(ctx);
+  if (tri) {
+    KTimer kt(ctx, KC_EPI);
+    k_triangulate_batch<<<dim3((cap + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(np1, np2, d_res, cap, d_inliers, d_pts3d);
+    MVO_CHECK_LAUNCH(ctx);
+  }
+  return MVO_OK;
 }
 
 // first half: everything up to the device-to-host copies, enqueued on ctx->stream (the caller may have pointed that at a side
@@ -203,7 +273,7 @@ int mvo_epi_essential_begin(mvo_ctx *ctx, const float *pts1, const float *pts2, 
   k_epi_score<<<grid, 256, smem, ctx->stream>>>(d1, d2, n, cam, thr2, H, dE, dvalid, dcnt); }
   MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, sizeof(EpiFinSmem), k_epi_finish, d1, d2, n, cam, thr2, H, (const double *)dE, (const int32_t *)dcnt, dout, dout_i, dinl)); }
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, 1, sizeof(EpiFinSmem), k_epi_finish, d1, d2, n, cam, thr2, H, (const double *)dE, (const int32_t *)dcnt, dout, dout_i, dinl)); }
   MVO_CHECK_LAUNCH(ctx);
   if (want_pose) {
     KTimer kt(ctx, KC_EPI);
@@ -324,7 +394,7 @@ int mvo_epi_homography_begin(mvo_ctx *ctx, const float *pts1, const float *pts2,
   k_homo_score<<<grid, 256, smem, ctx->stream>>>(d1, d2, n, cam, thr2, H, dH, dvalid, dcnt); }
   MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, sizeof(HomoFinSmem), k_homo_finish, d1, d2, n, cam, thr2, H, (const double *)dH, (const int32_t *)dcnt, dout, dout_i, dinl)); }
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, 1, sizeof(HomoFinSmem), k_homo_finish, d1, d2, n, cam, thr2, H, (const double *)dH, (const int32_t *)dcnt, dout, dout_i, dinl)); }
   MVO_CHECK_LAUNCH(ctx);
   double *h_out = (double *)(h + al((size_t)n * 16));
   int32_t *h_inl = (int32_t *)((uint8_t *)h_out + 512);

@@ -13,11 +13,13 @@ __device__ __forceinline__ uint64_t splitmix64e(uint64_t x) {
 
 struct EpiCam { double f, cx, cy; };      // findEssentialMat(focal, pp): one focal length (epipolar_geometry.cpp:26-27)
 
-__global__ void __launch_bounds__(128)
-k_epi_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, uint64_t seed, int H,
-                 double *__restrict__ Es, int32_t *__restrict__ valid) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= H) return;
+// The kernel bodies below are device functions that the single-pair kernels and their batched counterparts (one pair per
+// blockIdx.y, or one cluster per pair for the finish; mvo_esti_motion_by_essential_batch_dev) both call: the arithmetic exists
+// once, so a pair of a batch gets the bits of a single call on the same points.
+
+// hypothesis h: counter-based minimal sample of 8 distinct correspondences, epi::essential_from_8
+__device__ __forceinline__ void epi_hypothesis(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, uint64_t seed,
+                                               int h, double *__restrict__ Es, int32_t *__restrict__ valid) {
   int idx[8];
   uint64_t ctr = 0;
   for (int k = 0; k < 8; ++k)
@@ -42,9 +44,18 @@ k_epi_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int
   valid[h] = ok ? 1 : -reason;             // <= 0: rejected sample (the reason is kept for MVO_EPI_DEBUG)
 }
 
-__global__ void __launch_bounds__(256)
-k_epi_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
-            const double *__restrict__ Es, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
+__global__ void __launch_bounds__(128)
+k_epi_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, uint64_t seed, int H,
+                 double *__restrict__ Es, int32_t *__restrict__ valid) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= H) return;
+  epi_hypothesis(p1, p2, n, cam, seed, h, Es, valid);
+}
+
+// Sampson consensus of hypotheses cta * warps + warp, strided by ncta * warps; the CTA stages the n points once
+__device__ __forceinline__ void epi_score_run(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
+                                              const double *__restrict__ Es, const int32_t *__restrict__ valid, int32_t *__restrict__ counts,
+                                              int cta, int ncta) {
   EPI_DYN_SMEM(double, s_pt);         // [n][4] calibrated coordinates x1 y1 x2 y2
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     s_pt[4 * i] = ((double)p1[2 * i] - cam.cx) / cam.f; s_pt[4 * i + 1] = ((double)p1[2 * i + 1] - cam.cy) / cam.f;
@@ -52,7 +63,7 @@ k_epi_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, E
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  for (int h = blockIdx.x * wpb + warp; h < H; h += gridDim.x * wpb) {
+  for (int h = cta * wpb + warp; h < H; h += ncta * wpb) {
     if (valid[h] <= 0) { if (lane == 0) counts[h] = -1; continue; }
     double E[9];
     for (int q = 0; q < 9; ++q) E[q] = Es[(size_t)h * 9 + q];
@@ -62,6 +73,12 @@ k_epi_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, E
     for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
     if (lane == 0) counts[h] = c;
   }
+}
+
+__global__ void __launch_bounds__(256)
+k_epi_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
+            const double *__restrict__ Es, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
+  epi_score_run(p1, p2, n, cam, thr2, H, Es, valid, counts, blockIdx.x, gridDim.x);
 }
 
 constexpr int EFIN_T = 256;       // 255 registers per thread: the 20 (54) Gauss-Newton accumulators stay in registers (1024 threads = 64 registers spilled them)
@@ -214,10 +231,9 @@ struct EpiFinSmem {
   int cnt[EFIN_T / 32], best, stop, ipart[4];
 };
 
-__global__ void __launch_bounds__(EFIN_T)
-k_epi_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
-             const double *__restrict__ Es, const int32_t *__restrict__ counts, double *__restrict__ out_d,
-             int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
+__device__ __forceinline__ void epi_finish_run(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
+                                               const double *__restrict__ Es, const int32_t *__restrict__ counts, double *__restrict__ out_d,
+                                               int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
   EPI_DYN_SMEM(double, smraw);
   EpiFinSmem &S = *reinterpret_cast<EpiFinSmem *>(smraw);
   cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
@@ -410,13 +426,19 @@ k_epi_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, 
   cluster.sync();                                    // no CTA leaves while another still reads its shared memory
 }
 
+__global__ void __launch_bounds__(EFIN_T)
+k_epi_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
+             const double *__restrict__ Es, const int32_t *__restrict__ counts, double *__restrict__ out_d,
+             int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
+  epi_finish_run(p1, p2, n, cam, thr2, H, Es, counts, out_d, out_i, inl);
+}
+
 // recoverPose (calib3d five-point.cpp): triangulate every inlier with [I|0] and each of (R1,t) (R2,t) (R1,-t) (R2,-t); a point
 // votes for a candidate when its depth is in (0, 50) in both cameras.  One thread per (inlier, candidate); out_i[8 + c] += votes.
-__global__ void __launch_bounds__(256)
-k_epi_vote(const float *__restrict__ p1, const float *__restrict__ p2, EpiCam cam, const double *__restrict__ out_d,
-           int32_t *__restrict__ out_i, const int32_t *__restrict__ inl) {
+__device__ __forceinline__ void epi_vote_run(const float *__restrict__ p1, const float *__restrict__ p2, EpiCam cam, const double *__restrict__ out_d,
+                                             int32_t *__restrict__ out_i, const int32_t *__restrict__ inl, int cta) {
   const int n_in = out_i[0];
-  const int j = blockIdx.x * 64 + (threadIdx.x >> 2), c = threadIdx.x & 3;
+  const int j = cta * 64 + (threadIdx.x >> 2), c = threadIdx.x & 3;
   bool ok = false;
   if (j < n_in) {
     const int i = inl[j];
@@ -443,12 +465,15 @@ k_epi_vote(const float *__restrict__ p1, const float *__restrict__ p2, EpiCam ca
   }
 }
 
-__global__ void __launch_bounds__(128)
-k_triangulate(const float *__restrict__ np1, const float *__restrict__ np2, const int32_t *__restrict__ inl, int n_in,
-              const double *__restrict__ Rt /* 9 + 3 */, float *__restrict__ out) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n_in) return;
-  const int i = inl ? inl[j] : j;                 // no list: every correspondence (mvo_epi_essential_ex)
+__global__ void __launch_bounds__(256)
+k_epi_vote(const float *__restrict__ p1, const float *__restrict__ p2, EpiCam cam, const double *__restrict__ out_d,
+           int32_t *__restrict__ out_i, const int32_t *__restrict__ inl) {
+  epi_vote_run(p1, p2, cam, out_d, out_i, inl, blockIdx.x);
+}
+
+// doTriangulation of correspondence i into row j of out
+__device__ __forceinline__ void epi_triangulate_one(const float *__restrict__ np1, const float *__restrict__ np2, int i,
+                                                    const double *__restrict__ Rt /* 9 + 3 */, float *__restrict__ out, int j) {
   const double P0[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
   double P[12];
   for (int r = 0; r < 3; ++r) { P[4 * r] = Rt[3 * r]; P[4 * r + 1] = Rt[3 * r + 1]; P[4 * r + 2] = Rt[3 * r + 2]; P[4 * r + 3] = Rt[9 + r]; }
@@ -457,6 +482,132 @@ k_triangulate(const float *__restrict__ np1, const float *__restrict__ np2, cons
   // pts4d is CV_32F for float input points; the reference divides by the fourth coordinate in float (:161-168)
   const float x = (float)X[0], y = (float)X[1], z = (float)X[2], w = (float)X[3];
   out[3 * j] = x / w; out[3 * j + 1] = y / w; out[3 * j + 2] = z / w;
+}
+
+__global__ void __launch_bounds__(128)
+k_triangulate(const float *__restrict__ np1, const float *__restrict__ np2, const int32_t *__restrict__ inl, int n_in,
+              const double *__restrict__ Rt /* 9 + 3 */, float *__restrict__ out) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_in) return;
+  const int i = inl ? inl[j] : j;                 // no list: every correspondence (mvo_epi_essential_ex)
+  epi_triangulate_one(np1, np2, i, Rt, out, j);
+}
+
+// ------------------------------------------------------------------------------------ batch of frame pairs
+// mvo_esti_motion_by_essential_batch_dev: the kernels above for n_pairs matched frame pairs at once.  Pair p's scratch rows:
+// points at p * cap, hypotheses at p * H, finish outputs at p * EPIB_OUT_D / p * EPIB_OUT_I.  pn[p] (written by k_epi_gather):
+// the pair's correspondence count, or MVO_ERR_INVALID_ARG; every later kernel skips a pair whose pn is below 8.
+constexpr int EPIB_OUT_D = 32, EPIB_OUT_I = 16;
+
+// One CTA per pair: checks the frame indices, the match count and every match's keypoint indices before reading through them,
+// then writes pts1 / pts2 (pixels) and, for the triangulation, the normalised-plane points of two_view.cpp (pixel2CamNormPlane).
+__global__ void __launch_bounds__(256)
+k_epi_gather(const mvo_keypoint *__restrict__ kpts, const int32_t *__restrict__ kcounts, int batch, int cap, const int2 *__restrict__ pairs,
+             const mvo_dmatch *__restrict__ matches, const int32_t *__restrict__ n_matches, double fx, double fy, double cx, double cy,
+             float *__restrict__ p1, float *__restrict__ p2, float *__restrict__ np1, float *__restrict__ np2, int32_t *__restrict__ pn) {
+  __shared__ int s_bad;
+  const int pair = blockIdx.x;
+  const int2 fr = pairs[pair];
+  if (threadIdx.x == 0) s_bad = 0;
+  __syncthreads();
+  if (fr.x < 0 || fr.x >= batch || fr.y < 0 || fr.y >= batch) { if (threadIdx.x == 0) pn[pair] = MVO_ERR_INVALID_ARG; return; }
+  const int n = n_matches[pair];
+  if (n < 0 || n > cap) { if (threadIdx.x == 0) pn[pair] = MVO_ERR_INVALID_ARG; return; }
+  const int cq = min(max(kcounts[fr.x], 0), cap), ct = min(max(kcounts[fr.y], 0), cap);
+  const mvo_keypoint *kq = kpts + (size_t)fr.x * cap, *kt = kpts + (size_t)fr.y * cap;
+  const size_t o = (size_t)pair * cap * 2;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const mvo_dmatch m = matches[(size_t)pair * cap + i];
+    if (m.query_idx < 0 || m.query_idx >= cq || m.train_idx < 0 || m.train_idx >= ct) { atomicOr(&s_bad, 1); continue; }
+    const float x1 = kq[m.query_idx].x, y1 = kq[m.query_idx].y, x2 = kt[m.train_idx].x, y2 = kt[m.train_idx].y;
+    p1[o + 2 * i] = x1; p1[o + 2 * i + 1] = y1; p2[o + 2 * i] = x2; p2[o + 2 * i + 1] = y2;
+    if (np1) {
+      np1[o + 2 * i] = (float)(((double)x1 - cx) / fx); np1[o + 2 * i + 1] = (float)(((double)y1 - cy) / fy);
+      np2[o + 2 * i] = (float)(((double)x2 - cx) / fx); np2[o + 2 * i + 1] = (float)(((double)y2 - cy) / fy);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) pn[pair] = s_bad ? MVO_ERR_INVALID_ARG : n;
+}
+
+__global__ void __launch_bounds__(128)
+k_epi_hypotheses_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, EpiCam cam,
+                       uint64_t seed, int H, double *__restrict__ Es, int32_t *__restrict__ valid) {
+  const int pair = blockIdx.y, h = blockIdx.x * blockDim.x + threadIdx.x, n = pn[pair];
+  if (h >= H || n < 8) return;
+  epi_hypothesis(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, seed, h, Es + (size_t)pair * H * 9, valid + (size_t)pair * H);
+}
+
+// gridDim.x CTAs per pair (blockIdx.y); each stages only its own pair's points
+__global__ void __launch_bounds__(256)
+k_epi_score_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, EpiCam cam, double thr2,
+                  int H, const double *__restrict__ Es, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
+  const int pair = blockIdx.y, n = pn[pair];
+  if (n < 8) return;
+  const size_t oh = (size_t)pair * H;
+  epi_score_run(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, thr2, H, Es + oh * 9, valid + oh, counts + oh, blockIdx.x, gridDim.x);
+}
+
+// one cluster per pair: CTAs [pair * csize, (pair + 1) * csize) along x, the cluster size and rank split of k_epi_finish
+__global__ void __launch_bounds__(EFIN_T)
+k_epi_finish_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, EpiCam cam, double thr2,
+                   int H, const double *__restrict__ Es, const int32_t *__restrict__ counts, double *__restrict__ out_d,
+                   int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
+  const int pair = blockIdx.x / cooperative_groups::this_cluster().num_blocks(), n = pn[pair];
+  if (n < 8) return;                                 // the whole cluster
+  const size_t op = (size_t)pair * cap, oh = (size_t)pair * H;
+  epi_finish_run(p1 + op * 2, p2 + op * 2, n, cam, thr2, H, Es + oh * 9, counts + oh, out_d + (size_t)pair * EPIB_OUT_D,
+                 out_i + (size_t)pair * EPIB_OUT_I, inl + op);
+}
+
+__global__ void __launch_bounds__(256)
+k_epi_vote_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, EpiCam cam,
+                 const double *__restrict__ out_d, int32_t *__restrict__ out_i, const int32_t *__restrict__ inl) {
+  const int pair = blockIdx.y;
+  if (pn[pair] < 8) return;
+  const size_t op = (size_t)pair * cap;
+  epi_vote_run(p1 + op * 2, p2 + op * 2, cam, out_d + (size_t)pair * EPIB_OUT_D, out_i + (size_t)pair * EPIB_OUT_I, inl + op, blockIdx.x);
+}
+
+// recoverPose's choice among (R1,t) (R2,t) (R1,-t) (R2,-t) and t /= |t|, as mvo_epi_essential_end does on the host: the first
+// candidate whose vote count is a maximum.  |t| without contraction (the host's sum of three products), so t keeps the host's bits.
+// One thread per pair; a failed pair gets its status and nothing else.
+__global__ void __launch_bounds__(128)
+k_epi_pick(const int32_t *__restrict__ pn, int n_pairs, const double *__restrict__ out_d, const int32_t *__restrict__ out_i,
+           mvo_two_view_result *__restrict__ res) {
+  const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pair >= n_pairs) return;
+  const int n = pn[pair];
+  mvo_two_view_result &r = res[pair];
+  if (n < 0) { r.status = n; return; }
+  const int32_t *oi = out_i + (size_t)pair * EPIB_OUT_I;
+  if (n < 8 || oi[0] < 8) { r.status = MVO_ERR_DEGENERATE; return; }
+  const double *od = out_d + (size_t)pair * EPIB_OUT_D;
+  const int32_t *g = oi + 8;
+  int pick = 3;
+  if (g[0] >= g[1] && g[0] >= g[2] && g[0] >= g[3]) pick = 0;
+  else if (g[1] >= g[0] && g[1] >= g[2] && g[1] >= g[3]) pick = 1;
+  else if (g[2] >= g[0] && g[2] >= g[1] && g[2] >= g[3]) pick = 2;
+  const double *tt = od + 27, sg = pick < 2 ? 1.0 : -1.0;
+  const double nt = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(tt[0], tt[0]), __dmul_rn(tt[1], tt[1])), __dmul_rn(tt[2], tt[2])));
+  const double *Rp = od + ((pick & 1) ? 18 : 9);
+  for (int q = 0; q < 9; ++q) { r.E[q] = od[q]; r.R[q] = Rp[q]; }
+  for (int q = 0; q < 3; ++q) r.t[q] = __dmul_rn(sg, tt[q]) / nt;
+  r.status = MVO_OK; r.n_matches = n; r.n_inliers = oi[0]; r.votes = g[pick];
+}
+
+// doTriangulation of every pair's inliers with that pair's (R, t)
+__global__ void __launch_bounds__(128)
+k_triangulate_batch(const float *__restrict__ np1, const float *__restrict__ np2, const mvo_two_view_result *__restrict__ res, int cap,
+                    const int32_t *__restrict__ inl, float *__restrict__ out) {
+  const int pair = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  const mvo_two_view_result &r = res[pair];
+  if (r.status != MVO_OK || j >= r.n_inliers) return;
+  double Rt[12];
+  for (int q = 0; q < 9; ++q) Rt[q] = r.R[q];
+  for (int q = 0; q < 3; ++q) Rt[9 + q] = r.t[q];
+  const size_t op = (size_t)pair * cap;
+  epi_triangulate_one(np1 + op * 2, np2 + op * 2, inl[op + j], Rt, out + op * 3, j);
 }
 
 // ---------------------------------------------------------------------------------------------------- homography

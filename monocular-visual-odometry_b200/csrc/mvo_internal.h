@@ -98,6 +98,9 @@ struct mvo_ctx {
   PinBuf match_h;
   // batched matchFeatures (mvo_match_features_batch_dev): partial winners, merge tickets, packed keys of every pair
   DevBuf matchb_part, matchb_tickets, matchb_keys;
+  // batched essential-matrix motion (mvo_esti_motion_by_essential_batch_dev): points, hypotheses, counts and finish outputs of
+  // every pair; its own block, so that it never aliases the single-pair jobs' d_a / d_e that may run on the side stream
+  DevBuf epib_buf;
 
   // timing
   uint32_t timing_mask = 0;

@@ -22,6 +22,11 @@ KEYPOINT_DTYPE = np.dtype(
 DMATCH_DTYPE = np.dtype(
     [("query_idx", "<i4"), ("train_idx", "<i4"), ("img_idx", "<i4"), ("distance", "<f4")])
 assert KEYPOINT_DTYPE.itemsize == 28 and DMATCH_DTYPE.itemsize == 16
+# mvo_two_view_result (esti_motion_by_essential_batch_dev): one record per frame pair
+TWO_VIEW_RESULT_DTYPE = np.dtype(
+    [("status", "<i4"), ("n_matches", "<i4"), ("n_inliers", "<i4"), ("votes", "<i4"), ("E", "<f8", (9,)), ("R", "<f8", (9,)),
+     ("t", "<f8", (3,))])
+assert TWO_VIEW_RESULT_DTYPE.itemsize == 184
 
 MVO_OK = 0
 ERR_NAMES = {0: "MVO_OK", -1: "MVO_ERR_INVALID_ARG", -2: "MVO_ERR_NO_DEVICE", -3: "MVO_ERR_CUDA",
@@ -103,6 +108,7 @@ SIGNATURES = {
     "mvo_select_uniform_kpts_by_grid": (_i, [_vp, _vp, _pi, _i, _i]),
     "mvo_orb_extract_batch_dev": (_i, [_vp, _vp, _i, _i, _i, _i, _sz, _sz, _vp, _vp, _vp, _i]),
     "mvo_match_features_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _f, _vp, _vp]),
+    "mvo_esti_motion_by_essential_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, C.c_double, _vp, _vp, _vp]),
     "mvo_match_hamming_nn": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "mvo_match_hamming_knn2": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "mvo_match_radius_sad": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _f, _vp, _pi]),
@@ -305,6 +311,16 @@ class Context:
         pair p's matches land at d_out + p * cap records, their count (or MVO_ERR_INVALID_ARG for a bad pair) in d_n_out[p]."""
         self._chk(self.lib.mvo_match_features_batch_dev(self.h, _ptr(d_kpts), _ptr(d_desc), _ptr(d_counts), batch, cap, _ptr(d_pairs),
                                                         n_pairs, method_index, C.c_float(radius), _ptr(d_out), _ptr(d_n_out)))
+
+    def esti_motion_by_essential_batch_dev(self, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K, threshold,
+                                           d_res, d_inliers, d_pts3d=None):
+        """estiMotionByEssential (+ doTriangulation when d_pts3d is given) for n_pairs matched frame pairs of a batched
+        extraction, all device pointers except K (host 3x3): pair p's TWO_VIEW_RESULT_DTYPE record in d_res[p], its inlier
+        indices at d_inliers + p * cap, its triangulated inliers at d_pts3d + p * cap * 3."""
+        K = _c(K, np.float64)
+        self._chk(self.lib.mvo_esti_motion_by_essential_batch_dev(self.h, _ptr(d_kpts), _ptr(d_counts), batch, cap, _ptr(d_pairs), n_pairs,
+                                                                  _ptr(d_matches), _ptr(d_n_matches), _ptr(K), float(threshold), _ptr(d_res),
+                                                                  _ptr(d_inliers), _ptr(d_pts3d)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):
