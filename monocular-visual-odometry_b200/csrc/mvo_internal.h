@@ -1,8 +1,11 @@
 // Internal declarations shared by the CUDA translation units of libmvo.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <string.h>
 #include <string>
 #include <vector>
 #include "mvo.h"
@@ -128,6 +131,34 @@ struct KTimer {
 int mvo_reserve(mvo_ctx *ctx, DevBuf &b, size_t bytes);
 int mvo_reserve_pinned(mvo_ctx *ctx, PinBuf &b, size_t bytes);
 
+// Host arithmetic on rigid transforms (4x4 row-major doubles) shared by the tracker and the VO state machine, in the reference's
+// operation order: tracker.cpp and vo_pipeline.cpp get the same bits.
+static inline void set_identity(double *T) { memset(T, 0, 16 * sizeof(double)); T[0] = T[5] = T[10] = T[15] = 1; }
+static inline void inv_rigid(const double *T, double *Ti) {        // [R t; 0 1]^-1 = [R^T, -R^T t]; Ti may be T
+  double r[16];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) r[i * 4 + j] = T[j * 4 + i];
+  for (int i = 0; i < 3; ++i) r[i * 4 + 3] = -(r[i * 4] * T[3] + r[i * 4 + 1] * T[7] + r[i * 4 + 2] * T[11]);
+  r[12] = r[13] = r[14] = 0; r[15] = 1;
+  memcpy(Ti, r, sizeof r);
+}
+static inline void rt_to_T(const double *R, const double *t, double *T) {      // basics::convertRt2T
+  for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) T[i * 4 + j] = R[i * 3 + j]; T[i * 4 + 3] = t[i]; }
+  T[12] = T[13] = T[14] = 0; T[15] = 1;
+}
+// basics::preTranslatePoint3f: T(row, j) * p[j] accumulated in double over j = 0..3, narrowed to Point3f
+static inline void pre_translate(const float *p, const double *T, float *out) {
+  const double p0 = p[0], p1 = p[1], p2 = p[2];
+  for (int r = 0; r < 3; ++r) {
+    double a = 0;
+    a += T[r * 4] * p0; a += T[r * 4 + 1] * p1; a += T[r * 4 + 2] * p2; a += T[r * 4 + 3] * 1.0;
+    out[r] = (float)a;
+  }
+}
+static inline double trans_dist(const double *Ta, const double *Tb) {
+  const double dx = Ta[3] - Tb[3], dy = Ta[7] - Tb[7], dz = Ta[11] - Tb[11];
+  return sqrt(dx * dx + dy * dy + dz * dz);
+}
+
 // The tracker's device-resident frame buffer as the pose-only LM sees it (ba.cu: k_ba_pose<.., STORE>).
 // A buffered frame lives in one ring slot: its world->camera pose, its observation list (map point index +
 // pixel, in PnP-inlier order = Frame::inliers_to_mappt_connections_) and the length of that list.
@@ -142,31 +173,64 @@ struct MvoPoseStore {
   int cap, nslots, min_links;
   int slot[16];                // the window, newest first
   const int32_t *skip_flag;    // device flag: != 0 -> the kernel does nothing (PnP failed)
-  int32_t *out_info;           // [0] frames in the graph (0 = skipped), [1] edges, [2 + f] slot of frame f
+  int32_t *out_info;           // MvoTrackResultBlock::ba_graph
 };
 
-// track.cu: glue kernels of the device-resident tracking step
+// The match filter's record (MvoTrackFilter::d_info, MvoTrackResultBlock::filter): pairs in the filtered list, map points in view, status
+// (0 ok, 1 the host filter has to redo the frame), then MVO_TRACK_DEBUG counters: segments heapsorted at the depth limit, cycles of the
+// prologue / quicksort levels / epilogue, the longest heapsorted segment, the levels, and cycles / segments of level l < 7 at FI_LEVEL + 2 l
+enum MvoFilterInfo { FI_PAIRS, FI_CANDIDATES, FI_STATUS, FI_HEAP_SEGS, FI_CYC_PROLOGUE, FI_CYC_SORT, FI_CYC_EPILOGUE, FI_HEAP_MAX,
+                     FI_LEVELS, FI_LEVEL, FI_COUNT = 24 };
+
+// The device-resident tracker's per-frame result block: written by the kernels of a tracked frame, read back in one copy.
+// The offsets are fixed: bench.py counts these 768 bytes in a tracked frame's device-to-host traffic.
+struct MvoTrackResultBlock {
+  int32_t ba_skip;               // != 0: the window BA does nothing (PnP failed, or BA is off)
+  int32_t pad0[7];
+  int32_t pnp[3];                // model found, pnp_ok, consensus-set size
+  int32_t pad1[5];
+  int32_t ba_graph[18];          // frames in the graph (0 = skipped, < 0 = too large), edges, [2 + f] slot of frame f
+  int32_t pad2[6];
+  int32_t filter[FI_COUNT];      // MvoFilterInfo
+  double pose_before_ba[12];     // world->camera [R | t] of the frame before BA
+  double pad3[20];
+  double ba_stats[16];           // d_stats of mvo_ba_pose_store_launch
+  double pad4[16];
+};
+static_assert(offsetof(MvoTrackResultBlock, ba_skip) == 0, "result block layout");
+static_assert(offsetof(MvoTrackResultBlock, pnp) == 32, "result block layout");
+static_assert(offsetof(MvoTrackResultBlock, ba_graph) == 64, "result block layout");
+static_assert(offsetof(MvoTrackResultBlock, filter) == 160, "result block layout");
+static_assert(offsetof(MvoTrackResultBlock, pose_before_ba) == 256, "result block layout");
+static_assert(offsetof(MvoTrackResultBlock, ba_stats) == 512, "result block layout");
+static_assert(sizeof(MvoTrackResultBlock) == 768, "result block layout");
+
+// track.cu: k_track_glue's argument, passed by value (the field order and types are the kernel's parameter layout)
 struct MvoTrackGlue {
-  int mode;                      // 1 PnP ran on n pairs known to the host, 0 no PnP, 2 PnP ran on *n_pairs_dev pairs
-  int min_pnp;                   // mode 2: kMinPtsForPnP, tested on the device
+  int mode;                 // 1: a PnP ran (pose_io / out_i / inl valid); 0: too few pairs, only the fallback applies;
+                            // 2: a PnP was enqueued for *n_pairs_dev pairs — it counts only if that is >= min_pnp
+  int min_pnp;
   const int32_t *n_pairs_dev;
   int slot, cap, ba_enable, has_prev;
-  double max_dist, prev_twc[3], fallback[12];
+  double max_dist;          // max_possible_dist_to_prev_keyframe
+  double prev_twc[3];       // translation of the previous frame's T_w_c
+  double fallback[12];      // world->camera [R | t] the frame keeps when PnP fails (vo.cpp:376-379)
   const double *pose_io;
-  const int32_t *out_i, *inl, *pairs;
+  const int32_t *out_i, *inl;
+  const int2 *pairs;
   const mvo_keypoint *kpts;
-  int32_t *edge_map;
-  float *edge_obs;
-  int32_t *edge_kp;              // [ring][cap] keypoint index of every connection (the key of inliers_to_mappt_connections_)
-  int32_t *cnt;
-  double *pose;
-  int32_t *skip_flag, *res_i;
-  double *res_d;
-  const int32_t *map_ids;        // position in the map arrays -> map point id (what the frame buffer stores)
+  int32_t *edge_map;        // [ring][cap] map point ids
+  float2 *edge_obs;
+  int32_t *edge_kp;         // [ring][cap] keypoint index of every connection (the key of inliers_to_mappt_connections_)
+  const int32_t *map_ids;   // position in the map arrays -> map point id (what the frame buffer stores)
   // MapPoint::visible_times_ / matched_times_ increments (vo.cpp:44, :347), per position in the map arrays; nullptr = not counted
-  const uint8_t *vis;
+  const uint8_t *vis;       // in-view flags of this frame
   int nmap;
   int32_t *vis_cnt, *match_cnt;
+  int32_t *cnt;             // [ring]
+  double *pose;             // [ring][12]
+  int32_t *skip_flag, *res_i;  // MvoTrackResultBlock::ba_skip, ::pnp
+  double *res_d;               // MvoTrackResultBlock::pose_before_ba
 };
 int mvo_track_project_map(mvo_ctx *ctx, const float *d_map_pts, int nmap, const double *Tcw12, const double *K,
                           int rows, int cols, uint8_t *d_vis, float *d_cxy);
@@ -185,8 +249,7 @@ int mvo_track_kpt_colors(mvo_ctx *ctx, const mvo_keypoint *d_kpts, int n, const 
 int mvo_track_gather_pairs(mvo_ctx *ctx, const int32_t *d_pairs, int n, const int32_t *d_n, const float *d_map_pts,
                            const mvo_keypoint *d_kpts, float *d_p3, float *d_p2);
 int mvo_track_glue(mvo_ctx *ctx, const MvoTrackGlue &g);
-// thresholds of matchFeatures + removeDuplicatedMatches on the device; d_info (>= 24 ints): [0] pairs, [1] candidates,
-// [2] status, [4..22] phase / per-level cycle counters (MVO_TRACK_DEBUG)
+// thresholds of matchFeatures + removeDuplicatedMatches on the device; d_info: the FI_COUNT ints of MvoFilterInfo
 struct MvoTrackFilter {
   const uint32_t *d_keys;        // matcher keys of ALL map points
   uint8_t *d_vis;                // in-view flags: read, or written when Tcw12 != nullptr (projection done by the filter)

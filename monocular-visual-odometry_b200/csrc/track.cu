@@ -58,34 +58,7 @@ k_gather_pairs(const int2 *__restrict__ pairs, int n, const int32_t *__restrict_
   p2[2 * i] = kpts[pr.y].x; p2[2 * i + 1] = kpts[pr.y].y;
 }
 
-struct GlueArgs {
-  int mode;                 // 1: a PnP ran (pose_io / out_i / inl valid); 0: too few pairs, only the fallback applies;
-                            // 2: a PnP was enqueued for *n_pairs_dev pairs — it counts only if that is >= min_pnp
-  int min_pnp;
-  const int32_t *n_pairs_dev;
-  int slot, cap, ba_enable, has_prev;
-  double max_dist;          // max_possible_dist_to_prev_keyframe
-  double prev_twc[3];       // translation of the previous frame's T_w_c
-  Rt12 fallback;            // world->camera pose the frame keeps when PnP fails (vo.cpp:376-379)
-  const double *pose_io;
-  const int32_t *out_i, *inl;
-  const int2 *pairs;
-  const mvo_keypoint *kpts;
-  int32_t *edge_map;        // [ring][cap] map point ids
-  float2 *edge_obs;
-  int32_t *edge_kp;         // [ring][cap] keypoint indices
-  const int32_t *map_ids;   // position in the map arrays -> id
-  const uint8_t *vis;       // in-view flags of this frame (visible_times_++ of getMappointsInCurrentView_, vo.cpp:44)
-  int nmap;
-  int32_t *vis_cnt, *match_cnt;
-  int32_t *cnt;             // [ring]
-  double *pose;             // [ring][12]
-  int32_t *skip_flag;
-  int32_t *res_i;           // [0] model found, [1] pnp_ok, [2] consensus-set size
-  double *res_d;            // [0..11] world->camera pose of the frame before BA
-};
-
-__global__ void __launch_bounds__(1024) k_track_glue(GlueArgs a) {
+__global__ void __launch_bounds__(1024) k_track_glue(MvoTrackGlue a) {
   const int tid = threadIdx.x;
   pdl_wait();
   pdl_launch_dependents();
@@ -98,7 +71,7 @@ __global__ void __launch_bounds__(1024) k_track_glue(GlueArgs a) {
   if (tid == 0) {
     int ok = 0;
     double P[12];
-    for (int q = 0; q < 12; ++q) P[q] = a.fallback.v[q];
+    for (int q = 0; q < 12; ++q) P[q] = a.fallback[q];
     if (model) {
       ok = 1;
       for (int q = 0; q < 12; ++q) P[q] = a.pose_io[q];
@@ -108,7 +81,7 @@ __global__ void __launch_bounds__(1024) k_track_glue(GlueArgs a) {
       const double tz = -(P[2] * P[9] + P[5] * P[10] + P[8] * P[11]);
       const double dx = tx - a.prev_twc[0], dy = ty - a.prev_twc[1], dz = tz - a.prev_twc[2];
       if (a.has_prev && sqrt(dx * dx + dy * dy + dz * dz) >= a.max_dist) ok = 0;
-      if (!ok) for (int q = 0; q < 12; ++q) P[q] = a.fallback.v[q];
+      if (!ok) for (int q = 0; q < 12; ++q) P[q] = a.fallback[q];
     }
     for (int q = 0; q < 12; ++q) { a.pose[(size_t)a.slot * 12 + q] = P[q]; a.res_d[q] = P[q]; }
     a.cnt[a.slot] = n_in;                       // the connections are recorded before the jump test (vo.cpp:333-354)
@@ -193,17 +166,8 @@ int mvo_track_gather_pairs(mvo_ctx *ctx, const int32_t *d_pairs, int n, const in
 }
 
 int mvo_track_glue(mvo_ctx *ctx, const MvoTrackGlue &g) {
-  GlueArgs a;
-  a.mode = g.mode; a.min_pnp = g.min_pnp; a.n_pairs_dev = g.n_pairs_dev; a.slot = g.slot; a.cap = g.cap; a.ba_enable = g.ba_enable; a.has_prev = g.has_prev;
-  a.max_dist = g.max_dist;
-  for (int q = 0; q < 3; ++q) a.prev_twc[q] = g.prev_twc[q];
-  for (int q = 0; q < 12; ++q) a.fallback.v[q] = g.fallback[q];
-  a.pose_io = g.pose_io; a.out_i = g.out_i; a.inl = g.inl; a.pairs = (const int2 *)g.pairs; a.kpts = g.kpts;
-  a.edge_map = g.edge_map; a.edge_obs = (float2 *)g.edge_obs; a.edge_kp = g.edge_kp; a.cnt = g.cnt; a.pose = g.pose;
-  a.map_ids = g.map_ids; a.vis = g.vis; a.nmap = g.nmap; a.vis_cnt = g.vis_cnt; a.match_cnt = g.match_cnt;
-  a.skip_flag = g.skip_flag; a.res_i = g.res_i; a.res_d = g.res_d;
   KTimer kt(ctx, KC_TRACK);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, 1024, 0, 0, k_track_glue, a));
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, 1024, 0, 0, k_track_glue, g));
   ctx->launches++;
   return MVO_OK;
 }
@@ -232,10 +196,7 @@ int mvo_track_glue(mvo_ctx *ctx, const MvoTrackGlue &g) {
 //   * If a segment is still > 16 at the depth limit (libstdc++ would switch to heapsort: adversarial inputs
 //     only) the kernel reports status 1 and the host finishes the frame through the host path.
 // Parity: tests/test_tracker_gpu.py (same match lists as the host std::sort on every frame, all three methods).
-namespace {
-
 // (kernel text: track_filter.cuh)
-}  // namespace
 
 int mvo_track_match_filter(mvo_ctx *ctx, const MvoTrackFilter &f) {
   int cap = 2048;

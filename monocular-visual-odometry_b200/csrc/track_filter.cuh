@@ -43,7 +43,7 @@ struct FilterArgs {
   int nmap, nk, method, n_cap;
   double xg_ratio, lowe_ratio;
   int2 *pairs;              // out: (map index, keypoint index), sorted by keypoint index
-  int32_t *info;            // out: [0] pairs, [1] candidates (map points in view), [2] status (0 ok, 1 host path needed)
+  int32_t *info;            // out: the record of MvoFilterInfo (FI_PAIRS, FI_CANDIDATES, FI_STATUS, then the debug counters)
   // project == 1: getMappointsInCurrentView_ is evaluated here (methods 1/2: the matcher does not need the projections)
   int project;
   const float *map_pts;
@@ -194,7 +194,7 @@ __device__ __forceinline__ void match_filter_run(const FilterArgs &a, uint8_t *s
   if (tid == 0) { s_min = 0xFFFFFFFFu; s_status = 0; s_nseg[0] = s_nseg[1] = 0; s_heap_segs = 0; s_heap_max = 0; s_ndfs = 0; }
   pdl_wait();                       // first kernel of a tracked frame's chain (see launch_pdl.cuh)
   pdl_launch_dependents();
-  long long tph = clock64();        // phase cycle counters (thread 0) -> info[4..8]: prologue, compaction, sort levels, epilogue
+  long long tph = clock64();        // phase cycle counters (thread 0) -> info[FI_CYC_PROLOGUE + i]: prologue, sort levels, epilogue
 #define MF_MARK(i) do { if (tid == 0) { const long long t_ = clock64(); a.info[4 + (i)] = (int32_t)(t_ - tph); tph = t_; } } while (0)
   __syncthreads();
   // ---- thresholds (feature_match.cpp:179-196 for methods 1/3, :210-217 for method 2), ordered compaction ----
@@ -349,7 +349,7 @@ __device__ __forceinline__ void match_filter_run(const FilterArgs &a, uint8_t *s
     return;
   }
   MF_MARK(1);
-  if (tid == 0) { a.info[8] = level; a.info[3] = s_heap_segs; a.info[7] = s_heap_max; }     // [3], [7]: segments heapsorted at the depth limit, the longest
+  if (tid == 0) { a.info[8] = level; a.info[3] = s_heap_segs; a.info[7] = s_heap_max; }     // FI_LEVELS, FI_HEAP_SEGS, FI_HEAP_MAX
   // ---- final insertion sort is stable: of every run of equal keypoint indices the leftmost element survives ----
   for (int p = tid; p < n; p += MF_T) atomicMin(&best[arr[p] >> 16], ((uint32_t)p << 16) | (arr[p] & 0xFFFFu));
   __syncthreads();

@@ -22,7 +22,6 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
-#include <functional>
 #include <mutex>
 #include <stdlib.h>
 #include <math.h>
@@ -68,15 +67,6 @@ struct ExtractJob {
   std::vector<uint8_t> desc;
 };
 
-void inv_rigid(const double *T, double *Ti) {     // [R t; 0 1]^-1 = [R^T, -R^T t]
-  for (int i = 0; i < 3; ++i) {
-    for (int j = 0; j < 3; ++j) Ti[i * 4 + j] = T[j * 4 + i];
-    Ti[i * 4 + 3] = -(T[0 * 4 + i] * T[3] + T[1 * 4 + i] * T[7] + T[2 * 4 + i] * T[11]);
-  }
-  Ti[12] = Ti[13] = Ti[14] = 0;
-  Ti[15] = 1;
-}
-
 // camera->world 4x4  ->  world->camera [R (9) | t (3)], and back (g2o_ba.cpp:183-190, :298-305)
 void Twc_to_Rt12(const double *T, double *q) {
   for (int i = 0; i < 3; ++i) {
@@ -102,11 +92,6 @@ void rvec_to_R(const double *w, double *R) {      // cv::Rodrigues
   R[0] = 1 - B * (y * y + z * z); R[1] = -A * z + B * x * y;      R[2] = A * y + B * x * z;
   R[3] = A * z + B * x * y;       R[4] = 1 - B * (x * x + z * z); R[5] = -A * x + B * y * z;
   R[6] = -A * y + B * x * z;      R[7] = A * x + B * y * z;       R[8] = 1 - B * (x * x + y * y);
-}
-
-double trans_dist(const double *Ta, const double *Tb) {
-  const double dx = Ta[3] - Tb[3], dy = Ta[7] - Tb[7], dz = Ta[11] - Tb[11];
-  return sqrt(dx * dx + dy * dy + dz * dz);
 }
 
 double now_us() { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
@@ -166,10 +151,11 @@ struct mvo_tracker {
   uint8_t *d_keysvis[MVO_XSLOTS] = {nullptr, nullptr, nullptr};   // per extraction slot: [keys nmap*2 u32][vis nmap u8] — one D2H after the match
   int map_version = 0;                 // bumped by set_map: keys matched ahead of time against an older map are redone
   float *d_cxy = nullptr, *d_kxy = nullptr;
-  int32_t *d_pairs = nullptr, *d_edge_map = nullptr, *d_cnt = nullptr, *d_flags = nullptr;
-  float *d_edge_obs = nullptr;
-  double *d_pose = nullptr, *d_res = nullptr, *d_stats = nullptr;
-  uint8_t *h_pin = nullptr;            // pinned staging: [keys+vis][pairs][results]
+  int32_t *d_pairs = nullptr, *d_edge_map = nullptr, *d_cnt = nullptr;
+  float2 *d_edge_obs = nullptr;
+  double *d_pose = nullptr;
+  MvoTrackResultBlock *d_blk = nullptr;
+  uint8_t *h_pin = nullptr;            // pinned staging (StagingLayout)
   size_t h_pin_bytes = 0;
   // descriptors of the reference keyframe (mvo_vo: ref_), kept on the device so that a keyframe insertion matches against them
   // without an upload (mvo_trk_set_ref_desc / mvo_trk_keyframe_fetch)
@@ -284,6 +270,15 @@ bool use_device_path(const mvo_tracker *t) {
 
 size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
 
+// Pinned staging of the device-resident path for a map of nmap points (the first part is also the layout of an extraction slot's
+// d_keysvis): the matcher keys (nmap x 8 B) and in-view flags (nmap B), both read back in one copy by the host-filter redo; the pairs
+// the host filter sends to the device (<= nmap x 8 B) followed by its filter record; the result block; the pose ring (ring x 96 B).
+struct StagingLayout { size_t vis, pairs, result, ring; };
+StagingLayout staging_layout(int nmap) {
+  const size_t n = (size_t)std::max(nmap, 1), pairs = al256(n * 9), result = pairs + al256(n * 8 + 64);
+  return StagingLayout{n * 8, pairs, result, result + sizeof(MvoTrackResultBlock)};
+}
+
 // (Re)allocate / refresh the device-resident state.  Three blocks, each reallocated only when it has to grow (the map
 // changes at every keyframe once mvo_vo drives the tracker): the frame ring (keypoint capacity x ring size; holds the
 // buffered frames, so it is only rebuilt when those parameters change), the map arrays by position (capacity doubled on
@@ -308,9 +303,7 @@ int dev_alloc(mvo_tracker *t) {
     const size_t o_ekp = o;   o = al256(o + (size_t)ring * cap * 4);
     const size_t o_cnt = o;   o = al256(o + (size_t)ring * 4);
     const size_t o_pose = o;  o = al256(o + (size_t)ring * 96);
-    const size_t o_flags = o; o = al256(o + 256);       // [0] BA skip flag, [8..] res_i (3), [16..] out_info (2 + 16)
-    const size_t o_res = o;   o = al256(o + 256);       // res_d (12 doubles)
-    const size_t o_stats = o; o = al256(o + 256);       // BA stats (16 doubles)
+    const size_t o_blk = o;   o = al256(o + sizeof(MvoTrackResultBlock));
     const size_t o_ref = o;   o = al256(o + (size_t)cap * 32);
     uint8_t *nd = nullptr;
     MVO_CUDA(ctx, cudaMalloc(&nd, o));
@@ -319,9 +312,9 @@ int dev_alloc(mvo_tracker *t) {
     if (t->dev) cudaFree(t->dev);
     for (TrackedFrame &f : t->frames) f.slot = -1;      // frames buffered under the old layout leave the device-side BA window
     t->dev = nd; t->dev_cap = cap; t->dev_ring = ring;
-    t->d_kxy = (float *)(nd + o_kxy); t->d_edge_map = (int32_t *)(nd + o_emap); t->d_edge_obs = (float *)(nd + o_eobs);
+    t->d_kxy = (float *)(nd + o_kxy); t->d_edge_map = (int32_t *)(nd + o_emap); t->d_edge_obs = (float2 *)(nd + o_eobs);
     t->d_edge_kp = (int32_t *)(nd + o_ekp); t->d_cnt = (int32_t *)(nd + o_cnt); t->d_pose = (double *)(nd + o_pose);
-    t->d_flags = (int32_t *)(nd + o_flags); t->d_res = (double *)(nd + o_res); t->d_stats = (double *)(nd + o_stats);
+    t->d_blk = (MvoTrackResultBlock *)(nd + o_blk);
     t->d_ref_desc = nd + o_ref; t->n_ref = 0; t->ref_tag = -1;
     t->ring_host.assign((size_t)ring * 12, 0.0);
     t->spec.valid = false;
@@ -349,7 +342,7 @@ int dev_alloc(mvo_tracker *t) {
     for (int k = 0; k < MVO_XSLOTS; ++k) t->d_keysvis[k] = nd + o_kv[k];
     t->d_cxy = (float *)(nd + o_cxy); t->d_pairs = (int32_t *)(nd + o_pairs); t->d_map_ids = (int32_t *)(nd + o_ids);
     t->d_vis_cnt = (int32_t *)(nd + o_vc); t->d_match_cnt = (int32_t *)(nd + o_mc);
-    const size_t hb = al256((size_t)mcap * 9) + al256((size_t)mcap * 8 + 64) + al256((size_t)4096 * 96) + 1024;
+    const size_t hb = staging_layout(mcap).ring + (size_t)4096 * 96;      // a ring of the largest buffer_size a tracker accepts
     if (hb > t->h_pin_bytes) {
       if (t->h_pin) cudaFreeHost(t->h_pin);
       t->h_pin = nullptr;
@@ -381,6 +374,26 @@ int dev_alloc(mvo_tracker *t) {
     MVO_CUDA(ctx, cudaMemcpyAsync(t->d_alive, t->alive.data(), (size_t)n_ids, cudaMemcpyHostToDevice, ctx->stream));
   }
   MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));      // the extraction stream reads the map right away
+  return MVO_OK;
+}
+
+// pushFrameToBuff_ (vo.h:81-86): the new frame enters frames_buff_, the oldest leaves it beyond buffer_size.  in_ring: the frame takes
+// the next slot of the device frame ring (the host-array path keeps its frames on the host only)
+TrackedFrame &push_frame(mvo_tracker *t, bool in_ring) {
+  t->frames.emplace_back();
+  if ((int)t->frames.size() > t->prm.buffer_size) t->frames.pop_front();
+  TrackedFrame &f = t->frames.back();
+  if (in_ring) f.slot = (int)(t->frame_counter++ % (unsigned)t->dev_ring);
+  return f;
+}
+
+// n connections (map point id, keypoint index, pixel) of ring slot `slot` from position `first` on, host -> device
+int upload_links(mvo_tracker *t, int slot, int first, const int32_t *ids, const int32_t *kp_idx, const float *obs_xy, int n) {
+  mvo_ctx *ctx = t->ctx;
+  const size_t o = (size_t)slot * t->dev_cap + first;
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_map + o, ids, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_kp + o, kp_idx, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_obs + o, obs_xy, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
   return MVO_OK;
 }
 
@@ -456,7 +469,7 @@ extern "C" int mvo_test_match_filter_host(mvo_ctx *ctx, const uint32_t *keys, co
   int ncand = 0;
   host_match_filter(ctx->prm, method, nk > 0, keys, vis, nmap, v, &ncand);
   for (size_t i = 0; i < v.size(); ++i) { pairs[2 * i] = v[i].map; pairs[2 * i + 1] = v[i].train; }
-  info[0] = (int32_t)v.size(); info[1] = ncand; info[2] = 0;
+  info[FI_PAIRS] = (int32_t)v.size(); info[FI_CANDIDATES] = ncand; info[FI_STATUS] = 0;
   return MVO_OK;
 }
 
@@ -478,7 +491,7 @@ extern "C" int mvo_test_match_filter_dev(mvo_ctx *ctx, const uint32_t *keys, con
   if (rc == MVO_OK) {
     cudaMemcpyAsync(info, d + o_info, 48, cudaMemcpyDeviceToHost, ctx->stream);
     if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = mvo_fail(ctx, MVO_ERR_CUDA, "match filter kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-    else if (info[2] == 0 && info[0] > 0) cudaMemcpy(pairs, d + o_pairs, (size_t)info[0] * 8, cudaMemcpyDeviceToHost);
+    else if (info[FI_STATUS] == 0 && info[FI_PAIRS] > 0) cudaMemcpy(pairs, d + o_pairs, (size_t)info[FI_PAIRS] * 8, cudaMemcpyDeviceToHost);
   }
   cudaFree(d);
   return rc;
@@ -563,8 +576,7 @@ int mvo_tracker_create(mvo_ctx *ctx, const double *K, int rows, int cols, const 
     delete t;
     return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "tracker: bad parameters");
   }
-  memset(t->T_ref, 0, sizeof t->T_ref);
-  t->T_ref[0] = t->T_ref[5] = t->T_ref[10] = t->T_ref[15] = 1;
+  set_identity(t->T_ref);
   for (int k = 0; k < MVO_XSLOTS; ++k) {
     const int rc = mvo_create(&t->xctx[k], ctx->device, &ctx->prm);
     if (rc != MVO_OK) {
@@ -905,25 +917,17 @@ int mvo_trk_push_frame(mvo_tracker *t, const double *T_w_c, const int32_t *ids, 
   mvo_ctx *ctx = t->ctx;
   MVO_TRY(dev_alloc(t));
   if (n > t->dev_cap) return mvo_fail(ctx, MVO_ERR_CAPACITY, "tracker: %d connections exceed the keypoint capacity %d", n, t->dev_cap);
-  t->frames.emplace_back();
-  if ((int)t->frames.size() > t->prm.buffer_size) t->frames.pop_front();
-  TrackedFrame &cur = t->frames.back();
-  cur.slot = (int)(t->frame_counter++ % (unsigned)t->dev_ring);
+  TrackedFrame &cur = push_frame(t, true);
   cur.n_links = n;
   memcpy(cur.T_w_c, T_w_c, sizeof cur.T_w_c);
   double P[12];
   Twc_to_Rt12(T_w_c, P);
-  const size_t o = (size_t)cur.slot * t->dev_cap;
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
   MVO_CUDA(ctx, cudaMemcpyAsync(t->d_pose + (size_t)cur.slot * 12, P, sizeof P, cudaMemcpyHostToDevice, ctx->stream));
   if (t->ring_host.size() >= ((size_t)cur.slot + 1) * 12) memcpy(&t->ring_host[(size_t)cur.slot * 12], P, sizeof P);
   t->spec.valid = false;
   MVO_CUDA(ctx, cudaMemcpyAsync(t->d_cnt + cur.slot, &n, 4, cudaMemcpyHostToDevice, ctx->stream));
-  if (n > 0) {
-    MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_map + o, ids, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_kp + o, kp_idx, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_obs + 2 * o, obs_xy, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  }
+  if (n > 0) MVO_TRY(upload_links(t, cur.slot, 0, ids, kp_idx, obs_xy, n));
   MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   memcpy(t->T_prev, T_w_c, sizeof t->T_prev);
   t->has_prev = true;
@@ -937,12 +941,9 @@ int mvo_trk_append_links(mvo_tracker *t, int k, const int32_t *ids, const int32_
   TrackedFrame &f = t->frames[t->frames.size() - 1 - (size_t)k];
   if (n <= 0 || f.slot < 0) return MVO_OK;
   if (f.n_links + n > t->dev_cap) return mvo_fail(ctx, MVO_ERR_CAPACITY, "tracker: %d connections exceed the keypoint capacity %d", f.n_links + n, t->dev_cap);
-  const size_t o = (size_t)f.slot * t->dev_cap + f.n_links;
   const int total = f.n_links + n;
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_map + o, ids, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_kp + o, kp_idx, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_edge_obs + 2 * o, obs_xy, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_TRY(upload_links(t, f.slot, f.n_links, ids, kp_idx, obs_xy, n));
   MVO_CUDA(ctx, cudaMemcpyAsync(t->d_cnt + f.slot, &total, 4, cudaMemcpyHostToDevice, ctx->stream));
   MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   t->ref_copy_pending = false;
@@ -978,282 +979,289 @@ int mvo_trk_track(mvo_tracker *t, int slot, const double *T_guess, const double 
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// device-resident path
+// device-resident path: track_device runs the stages below over one DevFrame
 // ------------------------------------------------------------------------------------------------------------
-// Layout of the 768-byte result block (d_flags, d_res, d_stats are contiguous):
-//   int32 [0] BA skip flag   [8..10] model found, pnp_ok, inliers   [16..33] BA graph: frames, edges, slot of frame f
-//         [40..48] match filter: pairs, candidates, status, -, phase cycle counters
-//   +256: world->camera pose of the frame before BA (12 doubles)      +512: BA statistics (16 doubles)
-static int track_device(mvo_tracker *t, ExtractJob &job, int slot, double *T_w_c_out, mvo_track_result *res, int ref_k, int allow_spec) {
-  mvo_ctx *ctx = t->ctx;
-  // ring slot of the reference keyframe (the frame whose pose is the initial guess), looked up before this frame enters the buffer
-  int ref_slot = -1;
-  if (ref_k >= 1 && ref_k <= (int)t->frames.size()) ref_slot = t->frames[t->frames.size() - (size_t)ref_k].slot;
-  mvo_track_result r;
-  memset(&r, 0, sizeof r);
-  static const bool dbg = getenv("MVO_TRACK_DEBUG") != nullptr;
+namespace {
+
+struct DevFrame {
+  ExtractJob *job;
+  TrackedFrame *cur;
+  int nmap, nk, method, total;
+  int ref_slot;                      // ring slot of the reference keyframe when the guess is that frame's pose, else -1
+  StagingLayout pin;
+  uint8_t *d_keysvis, *d_vis;        // matcher keys and in-view flags of the extraction slot (the staging layout's first part)
+  const MvoTrackResultBlock *h_blk;  // the pinned copy of the result block
+  bool prematched, can_match, project_in_filter, filter_on_device;   // filter_on_device: not held off after a decline, nor MVO_TRACK_HOST_FILTER
+  double Tcw[12];                    // guess pose, world->camera
+  MvoPoseStore st;                   // the BA window of the last tail
+  bool counted;                      // visible_times_ / matched_times_ are accumulated by the first tail only
+  bool pnp_enqueued;                 // the PnP kernels of this frame were enqueued ahead of time (speculative chain head)
+};
+
+// a stage failed: the frame leaves the buffer again
+int drop_frame(mvo_tracker *t, int rc) { cudaStreamSynchronize(t->ctx->stream); t->frames.pop_back(); return rc; }
+
+// pushFrameToBuff_ (vo.h:81-86) with curr_->T_w_c_ = ref_->T_w_c_.clone() (vo_addFrame.cpp:74): initial guess = reference keyframe
+int frame_begin(mvo_tracker *t, DevFrame &fr, ExtractJob &job, int slot, int ref_k) {
   static const bool force_host_filter = getenv("MVO_TRACK_HOST_FILTER") != nullptr;     // test hook: the two-sync variant
+  MVO_CUDA(t->ctx, cudaSetDevice(t->ctx->device));
+  memset(&fr, 0, sizeof fr);
+  // ring slot of the reference keyframe (the frame whose pose is the initial guess), looked up before this frame enters the buffer
+  fr.ref_slot = ref_k >= 1 && ref_k <= (int)t->frames.size() ? t->frames[t->frames.size() - (size_t)ref_k].slot : -1;
+  fr.job = &job; fr.nmap = t->dev_nmap; fr.nk = job.nk; fr.method = t->prm.match_method;
+  fr.pin = staging_layout(fr.nmap);
+  fr.d_keysvis = t->d_keysvis[slot]; fr.d_vis = fr.d_keysvis + fr.pin.vis;
+  fr.h_blk = (const MvoTrackResultBlock *)(t->h_pin + fr.pin.result);
+  fr.prematched = job.matched && job.map_version == t->map_version && job.match_mode == (fr.method == 1 ? 0 : 1) && fr.method != 3;
+  fr.can_match = fr.nmap > 0 && fr.nk > 0 && !(fr.method == 2 && fr.nk < 2);
+  fr.filter_on_device = !force_host_filter && t->fused_holdoff == 0;
+  // methods 1/2: the matcher does not need the projections, so the in-view test is folded into the filter kernel
+  // (the keys of points outside the view are simply ignored there); method 3 gates on the projected pixel
+  fr.project_in_filter = fr.method != 3 && fr.filter_on_device;
+  fr.cur = &push_frame(t, true);
+  memcpy(fr.cur->T_w_c, t->T_ref, sizeof fr.cur->T_w_c);
+  fr.total = (int)t->frames.size();
+  Twc_to_Rt12(fr.cur->T_w_c, fr.Tcw);
+  // When the guess is the pose of a buffered frame, its world->camera form is taken from the pose ring as it is (host mirror here,
+  // device memory for a chain head enqueued ahead of time: the same twelve doubles) instead of inverting the inverse again.
+  if (fr.ref_slot >= 0 && t->ring_host.size() >= ((size_t)fr.ref_slot + 1) * 12) {
+    const double *rp = &t->ring_host[(size_t)fr.ref_slot * 12];
+    double dmax = 0;
+    for (int q = 0; q < 12; ++q) dmax = std::max(dmax, fabs(rp[q] - fr.Tcw[q]));
+    if (dmax < 1e-9) memcpy(fr.Tcw, rp, sizeof fr.Tcw);
+    else fr.ref_slot = -1;                   // the caller's guess is not that frame's pose: no ring pose, no speculation
+  } else fr.ref_slot = -1;
+  return MVO_OK;
+}
+
+// getMappointsInCurrentView_ + matchFeatures(map descriptors, frame descriptors) (vo.cpp:16-49, 283-289)
+int frame_match(mvo_tracker *t, DevFrame &fr) {
+  mvo_ctx *ctx = t->ctx;
+  if (fr.nmap <= 0) return MVO_OK;
+  if (!fr.project_in_filter)
+    MVO_TRY(mvo_track_project_map(ctx, t->d_map_pts, fr.nmap, fr.Tcw, t->K, t->rows, t->cols, fr.d_vis, t->d_cxy));
+  if (!fr.can_match) {
+    if (cudaMemsetAsync(fr.d_keysvis, 0xFF, (size_t)fr.nmap * 8, ctx->stream) != cudaSuccess) return mvo_fail(ctx, MVO_ERR_CUDA, "tracker: memset");
+  } else if (!fr.prematched) {       // prematched: the keys of every map point are there (unmasked: the filters ignore points outside the view)
+    if (fr.method == 3) MVO_TRY(mvo_track_kpt_xy(ctx, fr.job->d_k, fr.nk, t->d_kxy));
+    MVO_TRY(mvo_match_launch_masked(ctx, fr.method == 1 ? 0 : (fr.method == 2 ? 1 : 2), t->d_map_desc, t->d_cxy, fr.nmap, fr.job->d_d, t->d_kxy,
+                                    fr.nk, t->prm.match_radius, (uint32_t *)fr.d_keysvis, fr.project_in_filter ? nullptr : fr.d_vis));
+  }
+  return MVO_OK;
+}
+
+// The head of a frame's chain: the match filter (in-view test, thresholds, duplicate removal, PnP input arrays); side-effect free apart
+// from scratch buffers.  jb / kv: this frame and its keys + in-view flags, or the next one's for a head enqueued ahead of time; Tcw_host /
+// d_Tcw: the guess pose as a kernel argument or in device memory (neither: the in-view flags are there already).
+int enqueue_head(mvo_tracker *t, const DevFrame &fr, const ExtractJob &jb, uint8_t *kv, const double *Tcw_host, const double *d_Tcw, int *n_upper) {
+  *n_upper = std::min(fr.nmap, std::max(jb.nk, 0));
+  MvoTrackFilter f;
+  memset(&f, 0, sizeof f);
+  f.d_keys = (uint32_t *)kv; f.d_vis = kv + fr.pin.vis; f.nmap = fr.nmap; f.nk = jb.nk; f.method = fr.method;
+  f.d_pairs = t->d_pairs; f.d_info = t->d_blk->filter; f.d_map_pts = t->d_map_pts;
+  if (Tcw_host || d_Tcw) { f.Tcw12 = Tcw_host; f.d_Tcw12 = d_Tcw; f.K = t->K; f.rows = t->rows; f.cols = t->cols; }
+  if (*n_upper >= 4) {         // the filter writes the PnP input arrays itself
+    double *d_pose_io;
+    int32_t *d_out_i, *d_inl;
+    MVO_TRY(mvo_pnp_dev_buffers(t->ctx, *n_upper, &f.d_p3, &f.d_p2, &d_pose_io, &d_out_i, &d_inl));
+    f.d_kpts = jb.d_k;
+  }
+  return mvo_track_match_filter(t->ctx, f);
+}
+
+// The next prefetched frame's chain head (match filter + PnP), once its extraction and pre-match are done, with the guess pose read
+// from the ring slot of the reference keyframe, which this frame's BA may move
+int speculate_next_head(mvo_tracker *t, const DevFrame &fr) {
+  const int ns = (int)(t->n_consume % MVO_XSLOTS);
+  ExtractJob &nj = t->job[ns];
+  if (nj.want_host) return MVO_OK;
+  wait_job(t, ns);
+  if (nj.rc != MVO_OK || !nj.matched || nj.map_version != t->map_version || nj.match_mode != (fr.method == 1 ? 0 : 1) || nj.nk <= 0 ||
+      (fr.method == 2 && nj.nk < 2))
+    return MVO_OK;
+  int n_up = 0;
+  MVO_TRY(enqueue_head(t, fr, nj, t->d_keysvis[ns], nullptr, t->d_pose + (size_t)fr.ref_slot * 12, &n_up));
+  if (n_up >= 4) MVO_TRY(mvo_pnp_dev_run(t->ctx, n_up, t->K, &t->d_blk->filter[FI_PAIRS]));
+  t->spec = mvo_tracker::Spec{true, nj.serial, t->map_version, fr.ref_slot, fr.nmap, nj.nk, fr.method, n_up};
+  ++t->spec_issued;
+  return MVO_OK;
+}
+
+// Everything after the match filter: PnP (unless it went with the head), the glue kernel, the BA window, then ONE device-to-host copy of
+// the result block and the pose ring.  d_n != nullptr: the pair count lives on the device (n = its upper bound); otherwise n pairs are
+// in d_pairs.  gathered: the filter has written the PnP input arrays.  speculate: enqueue the next frame's chain head behind the copy.
+int enqueue_tail(mvo_tracker *t, DevFrame &fr, int n, const int32_t *d_n, bool gathered, bool speculate) {
+  mvo_ctx *ctx = t->ctx;
+  MvoTrackResultBlock *blk = t->d_blk;
+  MvoTrackGlue g;
+  memset(&g, 0, sizeof g);
+  const bool run_pnp = n >= 4 && (d_n != nullptr || n >= t->prm.min_pnp_points);
+  g.mode = run_pnp ? (d_n ? 2 : 1) : 0;
+  g.min_pnp = t->prm.min_pnp_points; g.n_pairs_dev = d_n;
+  g.slot = fr.cur->slot; g.cap = t->dev_cap; g.ba_enable = t->prm.ba_enable; g.has_prev = t->has_prev;
+  g.max_dist = t->prm.max_dist_to_prev;
+  if (t->has_prev) { g.prev_twc[0] = t->T_prev[3]; g.prev_twc[1] = t->T_prev[7]; g.prev_twc[2] = t->T_prev[11]; }
+  Twc_to_Rt12(t->has_prev ? t->T_prev : fr.cur->T_w_c, g.fallback);      // vo.cpp:376-379
+  g.pairs = (const int2 *)t->d_pairs; g.kpts = fr.job->d_k;
+  g.edge_map = t->d_edge_map; g.edge_obs = t->d_edge_obs; g.edge_kp = t->d_edge_kp; g.cnt = t->d_cnt; g.pose = t->d_pose;
+  g.skip_flag = &blk->ba_skip; g.res_i = blk->pnp; g.res_d = blk->pose_before_ba;
+  g.map_ids = t->d_map_ids; g.vis = fr.d_vis; g.nmap = fr.nmap;
+  // visible_times_ once per frame; matched_times_ by the tail whose PnP saw the pairs (a declined device filter hands
+  // its tail zero pairs, so the redo through the host filter is the one that counts the inliers)
+  if (t->count_stats && fr.nmap > 0) { g.match_cnt = t->d_match_cnt; if (!fr.counted) g.vis_cnt = t->d_vis_cnt; }
+  if (run_pnp) {
+    float *d_p3, *d_p2;
+    double *d_pose_io;
+    int32_t *d_out_i, *d_inl;
+    MVO_TRY(mvo_pnp_dev_buffers(ctx, n, &d_p3, &d_p2, &d_pose_io, &d_out_i, &d_inl));
+    g.pose_io = d_pose_io; g.out_i = d_out_i; g.inl = d_inl;
+    if (!gathered) MVO_TRY(mvo_track_gather_pairs(ctx, t->d_pairs, n, d_n, t->d_map_pts, fr.job->d_k, d_p3, d_p2));
+    if (!fr.pnp_enqueued) MVO_TRY(mvo_pnp_dev_run(ctx, n, t->K, d_n));
+    fr.pnp_enqueued = false;
+  }
+  MVO_TRY(mvo_track_glue(ctx, g));
+  // the BA window: newest min(ba_window, total-1) frames (vo.cpp:417-419); frames with < 3 links drop out on the
+  // device (:423-426), where the newest frame's link count is known
+  MvoPoseStore &st = fr.st;
+  memset(&st, 0, sizeof st);
+  if (run_pnp && t->prm.ba_enable) {
+    int e_upper = 0;
+    const int nba = std::min(t->prm.ba_window, fr.total - 1);
+    for (int b = fr.total - 1; b >= fr.total - nba; --b) {
+      if (t->frames[b].slot < 0) continue;         // tracked through the host-array path (parameters changed mid-sequence)
+      st.slot[st.nslots++] = t->frames[b].slot;
+      e_upper += (b == fr.total - 1) ? n : t->frames[b].n_links;
+    }
+    if (st.nslots > 0) {
+      st.map_pts = t->d_pos_by_id; st.alive = t->d_alive; st.n_ids = (int)t->alive.size(); st.edge_map = t->d_edge_map; st.edge_obs = t->d_edge_obs; st.cnt = t->d_cnt;
+      st.pose = t->d_pose; st.cap = t->dev_cap; st.min_links = 3; st.skip_flag = &blk->ba_skip; st.out_info = blk->ba_graph;
+      MVO_TRY(mvo_ba_pose_store_launch(ctx, st, e_upper, t->K[0], t->K[0], t->K[2], t->K[5], t->prm.information, ctx->prm.ba_iterations,
+                                       ctx->prm.ba_huber_delta > 0, ctx->prm.ba_huber_delta, t->prm.ba_step_tol, blk->ba_stats));
+    }
+  }
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->h_pin + fr.pin.result, blk, sizeof *blk, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->h_pin + fr.pin.ring, t->d_pose, (size_t)t->dev_ring * 96, cudaMemcpyDeviceToHost, ctx->stream));
+  if (!t->ev_result) MVO_CUDA(ctx, cudaEventCreateWithFlags(&t->ev_result, cudaEventDisableTiming));
+  MVO_CUDA(ctx, cudaEventRecord(t->ev_result, ctx->stream));
+  if (speculate) MVO_TRY(speculate_next_head(t, fr));
+  MVO_CUDA(ctx, cudaEventSynchronize(t->ev_result));
+  return MVO_OK;
+}
+
+// thresholds of matchFeatures (feature_match.cpp:179-217) and removeDuplicatedMatches (:241-260) on the host,
+// from the keys the matcher left on the device: the variant with a second synchronisation, used when the
+// device-side duplicate removal declines (list beyond its capacity, or libstdc++ would have left quicksort)
+int host_filter_redo(mvo_tracker *t, DevFrame &fr) {
+  mvo_ctx *ctx = t->ctx;
+  if (fr.nmap > 0) {
+    MVO_CUDA(ctx, cudaMemcpyAsync(t->h_pin, fr.d_keysvis, (size_t)fr.nmap * 9, cudaMemcpyDeviceToHost, ctx->stream));
+    MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  int ncand = 0;
+  host_match_filter(ctx->prm, fr.method, fr.can_match, (const uint32_t *)t->h_pin, t->h_pin + fr.pin.vis, fr.nmap, t->pairs, &ncand);
+  const int nm = (int)t->pairs.size();
+  int32_t *h_pairs = (int32_t *)(t->h_pin + fr.pin.pairs);
+  for (int i = 0; i < nm; ++i) { h_pairs[2 * i] = t->pairs[i].map; h_pairs[2 * i + 1] = t->pairs[i].train; }
+  int32_t *h_fi = h_pairs + 2 * (size_t)nm;          // the first three entries of the filter record
+  h_fi[FI_PAIRS] = nm; h_fi[FI_CANDIDATES] = ncand; h_fi[FI_STATUS] = 0;
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_pairs, h_pairs, (size_t)nm * 8, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(t->d_blk->filter, h_fi, 3 * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+  return enqueue_tail(t, fr, nm, nullptr, false, false);
+}
+
+// the frame's results from the pinned copy of the result block: match counts, the PnP pose (or the fallback), and the poses BA moved
+int read_results(mvo_tracker *t, DevFrame &fr, mvo_track_result &r) {
+  const MvoTrackResultBlock &b = *fr.h_blk;
+  const double *h_ring = (const double *)(t->h_pin + fr.pin.ring);
+  if (t->ring_host.size() >= (size_t)t->dev_ring * 12) memcpy(t->ring_host.data(), h_ring, (size_t)t->dev_ring * 96);
+  memset(&r, 0, sizeof r);
+  r.n_keypoints = fr.nk;
+  r.n_matches = b.filter[FI_PAIRS];
+  r.n_candidates = b.filter[FI_CANDIDATES];
+  r.pnp_ok = b.pnp[1] != 0;
+  r.n_inliers = fr.cur->n_links = b.pnp[2];
+  if (r.pnp_ok) Rt12_to_Twc(b.pose_before_ba, fr.cur->T_w_c);
+  else if (t->has_prev) memcpy(fr.cur->T_w_c, t->T_prev, sizeof fr.cur->T_w_c);
+  memcpy(r.T_w_c_pnp, fr.cur->T_w_c, sizeof r.T_w_c_pnp);
+  if (fr.st.nslots > 0 && r.pnp_ok) {
+    const int F = b.ba_graph[0];
+    if (F < 0) { t->frames.pop_back(); return mvo_fail(t->ctx, MVO_ERR_UNSUPPORTED, "tracker: BA graph exceeds the device-resident kernel"); }
+    for (int f = 0; f < F; ++f) {
+      const int s = b.ba_graph[2 + f];
+      for (int k = fr.total - 1; k >= 0; --k)
+        if (t->frames[k].slot == s) { Rt12_to_Twc(h_ring + (size_t)s * 12, t->frames[k].T_w_c); break; }
+    }
+    r.ba_frames = F;
+    r.ba_edges = b.ba_graph[1];
+    static const bool ba_dbg = getenv("MVO_BA_DEBUG") != nullptr;
+    const double *h_stats = b.ba_stats;
+    if (ba_dbg)
+      fprintf(stderr, "k_ba_pose(store): F=%d E=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f | "
+              "pdl_wait=%.0f setup=%.0f init=%.0f exit=%.0f kernel=%.0f\n", F, b.ba_graph[1], h_stats[2], h_stats[15], h_stats[7], h_stats[8],
+              h_stats[9], h_stats[10], h_stats[11], h_stats[12], h_stats[4], h_stats[5], h_stats[6], h_stats[13]);
+  }
+  return MVO_OK;
+}
+
+}  // namespace
+
+static int track_device(mvo_tracker *t, ExtractJob &job, int slot, double *T_w_c_out, mvo_track_result *res, int ref_k, int allow_spec) {
+  static const bool dbg = getenv("MVO_TRACK_DEBUG") != nullptr;
   static double acc[8] = {0};
   static int nacc = 0;
   double t0 = dbg ? now_us() : 0;
 #define TMARK(i) do { if (dbg) { const double t_ = now_us(); acc[i] += t_ - t0; t0 = t_; } } while (0)
-  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int nmap = t->dev_nmap, cap = t->dev_cap, nk = job.nk;
-  const int method = t->prm.match_method;
-  r.n_keypoints = nk;
-
-  // pushFrameToBuff_ (vo.h:81-86)
-  t->frames.emplace_back();
-  if ((int)t->frames.size() > t->prm.buffer_size) t->frames.pop_front();
-  TrackedFrame &cur = t->frames.back();
-  cur.slot = (int)(t->frame_counter++ % (unsigned)t->dev_ring);
-  // curr_->T_w_c_ = ref_->T_w_c_.clone()  (vo_addFrame.cpp:74): initial guess = reference keyframe
-  memcpy(cur.T_w_c, t->T_ref, sizeof cur.T_w_c);
-  const int total = (int)t->frames.size();
-
-  uint8_t *d_keysvis = t->d_keysvis[slot];
-  uint32_t *d_keys = (uint32_t *)d_keysvis;
-  uint8_t *d_vis = d_keysvis + (size_t)std::max(nmap, 1) * 8;
-  const bool prematched = job.matched && job.map_version == t->map_version && job.match_mode == (method == 1 ? 0 : 1) && method != 3;
-  int32_t *d_finfo = t->d_flags + 40, *d_res_i = t->d_flags + 8, *d_out_info = t->d_flags + 16;
-  uint8_t *h_out = t->h_pin + al256((size_t)std::max(nmap, 1) * 9) + al256((size_t)std::max(nmap, 1) * 8 + 64);
-  const int32_t *h_flags = (const int32_t *)h_out;
-  const bool can_match = nmap > 0 && nk > 0 && !(method == 2 && nk < 2);
-
-  // ---- getMappointsInCurrentView_ + matchFeatures(map descriptors, frame descriptors) (vo.cpp:16-49, 283-289) ----
-  auto fail = [&](int rc) { cudaStreamSynchronize(ctx->stream); t->frames.pop_back(); return rc; };
-  int rc = MVO_OK;
-  double Tcw[12];
-  Twc_to_Rt12(cur.T_w_c, Tcw);
-  // When the guess is the pose of a buffered frame, its world->camera form is taken from the pose ring as it is (host mirror here,
-  // device memory for a chain head enqueued ahead of time: the same twelve doubles) instead of inverting the inverse again.
-  if (ref_slot >= 0 && t->ring_host.size() >= ((size_t)ref_slot + 1) * 12) {
-    const double *rp = &t->ring_host[(size_t)ref_slot * 12];
-    double dmax = 0;
-    for (int q = 0; q < 12; ++q) dmax = std::max(dmax, fabs(rp[q] - Tcw[q]));
-    if (dmax < 1e-9) memcpy(Tcw, rp, sizeof Tcw);
-    else ref_slot = -1;                      // the caller's guess is not that frame's pose: no ring pose, no speculation
-  } else ref_slot = -1;
-  // methods 1/2: the matcher does not need the projections, so the in-view test is folded into the filter kernel
-  // (the keys of points outside the view are simply ignored there); method 3 gates on the projected pixel
-  const bool project_in_filter = method != 3 && !force_host_filter && t->fused_holdoff == 0;
-  if (nmap > 0) {
-    if (!project_in_filter) rc = mvo_track_project_map(ctx, t->d_map_pts, nmap, Tcw, t->K, t->rows, t->cols, d_vis, t->d_cxy);
-    if (rc == MVO_OK && can_match && prematched) {
-      // keys of every map point are already there (unmasked: the filter / host filter ignores points outside the view)
-    } else if (rc == MVO_OK && can_match) {
-      if (method == 3) rc = mvo_track_kpt_xy(ctx, job.d_k, nk, t->d_kxy);
-      if (rc == MVO_OK)
-        rc = mvo_match_launch_masked(ctx, method == 1 ? 0 : (method == 2 ? 1 : 2), t->d_map_desc, t->d_cxy, nmap, job.d_d, t->d_kxy, nk,
-                                     t->prm.match_radius, d_keys, project_in_filter ? nullptr : d_vis);
-    } else if (rc == MVO_OK) {
-      if (cudaMemsetAsync(d_keys, 0xFF, (size_t)nmap * 8, ctx->stream) != cudaSuccess) rc = mvo_fail(ctx, MVO_ERR_CUDA, "tracker: memset");
-    }
-    if (rc != MVO_OK) return fail(rc);
-  }
-
-  // ---- everything after the matcher: thresholds + duplicate removal, PnP, frame-buffer update, BA ----
-  // d_n != nullptr: the pair count lives on the device (n = its upper bound); otherwise n pairs are in d_pairs
-  MvoPoseStore st;
-  bool counted = false;            // visible_times_ / matched_times_ are accumulated by the first tail only
-  bool pnp_enqueued = false;       // the PnP kernels of this frame were enqueued ahead of time (speculative chain head)
-  std::function<int()> speculate;  // set by the fused path: enqueues the next frame's chain head behind this frame's result copy
-  auto enqueue_tail = [&](int n, const int32_t *d_n, bool gathered) -> int {
-    MvoTrackGlue g;
-    memset(&g, 0, sizeof g);
-    const bool run_pnp = n >= 4 && (d_n != nullptr || n >= t->prm.min_pnp_points);
-    g.mode = run_pnp ? (d_n ? 2 : 1) : 0;
-    g.min_pnp = t->prm.min_pnp_points; g.n_pairs_dev = d_n;
-    g.slot = cur.slot; g.cap = cap; g.ba_enable = t->prm.ba_enable; g.has_prev = t->has_prev;
-    g.max_dist = t->prm.max_dist_to_prev;
-    if (t->has_prev) { g.prev_twc[0] = t->T_prev[3]; g.prev_twc[1] = t->T_prev[7]; g.prev_twc[2] = t->T_prev[11]; }
-    Twc_to_Rt12(t->has_prev ? t->T_prev : cur.T_w_c, g.fallback);      // vo.cpp:376-379
-    g.pairs = t->d_pairs; g.kpts = job.d_k;
-    g.edge_map = t->d_edge_map; g.edge_obs = t->d_edge_obs; g.edge_kp = t->d_edge_kp; g.cnt = t->d_cnt; g.pose = t->d_pose;
-    g.skip_flag = t->d_flags; g.res_i = d_res_i; g.res_d = t->d_res;
-    g.map_ids = t->d_map_ids; g.vis = d_vis; g.nmap = nmap;
-    // visible_times_ once per frame; matched_times_ by the tail whose PnP saw the pairs (a declined device filter hands
-    // its tail zero pairs, so the redo through the host filter is the one that counts the inliers)
-    if (t->count_stats && nmap > 0) { g.match_cnt = t->d_match_cnt; if (!counted) g.vis_cnt = t->d_vis_cnt; }
-    int rc2 = MVO_OK;
-    if (run_pnp) {
-      float *d_p3, *d_p2;
-      double *d_pose_io;
-      int32_t *d_out_i, *d_inl;
-      rc2 = mvo_pnp_dev_buffers(ctx, n, &d_p3, &d_p2, &d_pose_io, &d_out_i, &d_inl);
-      if (rc2 == MVO_OK && !gathered) rc2 = mvo_track_gather_pairs(ctx, t->d_pairs, n, d_n, t->d_map_pts, job.d_k, d_p3, d_p2);
-      if (rc2 == MVO_OK && !pnp_enqueued) rc2 = mvo_pnp_dev_run(ctx, n, t->K, d_n);
-      pnp_enqueued = false;
-      g.pose_io = d_pose_io; g.out_i = d_out_i; g.inl = d_inl;
-    }
-    if (rc2 == MVO_OK) rc2 = mvo_track_glue(ctx, g);
-    // the BA window: newest min(ba_window, total-1) frames (vo.cpp:417-419); frames with < 3 links drop out on the
-    // device (:423-426), where the newest frame's link count is known
-    memset(&st, 0, sizeof st);
-    if (rc2 == MVO_OK && run_pnp && t->prm.ba_enable) {
-      int e_upper = 0;
-      const int nba = std::min(t->prm.ba_window, total - 1);
-      for (int b = total - 1; b >= total - nba; --b) {
-        if (t->frames[b].slot < 0) continue;         // tracked through the host-array path (parameters changed mid-sequence)
-        st.slot[st.nslots++] = t->frames[b].slot;
-        e_upper += (b == total - 1) ? n : t->frames[b].n_links;
-      }
-      if (st.nslots > 0) {
-        st.map_pts = t->d_pos_by_id; st.alive = t->d_alive; st.n_ids = (int)t->alive.size(); st.edge_map = t->d_edge_map; st.edge_obs = (const float2 *)t->d_edge_obs; st.cnt = t->d_cnt;
-        st.pose = t->d_pose; st.cap = cap; st.min_links = 3; st.skip_flag = t->d_flags; st.out_info = d_out_info;
-        rc2 = mvo_ba_pose_store_launch(ctx, st, e_upper, t->K[0], t->K[0], t->K[2], t->K[5], t->prm.information, ctx->prm.ba_iterations,
-                                       ctx->prm.ba_huber_delta > 0, ctx->prm.ba_huber_delta, t->prm.ba_step_tol, t->d_stats);
-      }
-    }
-    if (rc2 != MVO_OK) return rc2;
-    // one D2H: the result block + the pose ring
-    MVO_CUDA(ctx, cudaMemcpyAsync(h_out, t->d_flags, 768, cudaMemcpyDeviceToHost, ctx->stream));
-    MVO_CUDA(ctx, cudaMemcpyAsync(h_out + 768, t->d_pose, (size_t)t->dev_ring * 96, cudaMemcpyDeviceToHost, ctx->stream));
-    if (!t->ev_result) MVO_CUDA(ctx, cudaEventCreateWithFlags(&t->ev_result, cudaEventDisableTiming));
-    MVO_CUDA(ctx, cudaEventRecord(t->ev_result, ctx->stream));
-    if (speculate) { const int rcs = speculate(); if (rcs != MVO_OK) return rcs; }       // the next frame's chain head, behind this frame's results
-    MVO_CUDA(ctx, cudaEventSynchronize(t->ev_result));
-    return MVO_OK;
-  };
-
-  // thresholds of matchFeatures (feature_match.cpp:179-217) and removeDuplicatedMatches (:241-260) on the host,
-  // from the keys the matcher left on the device: the variant with a second synchronisation, used when the
-  // device-side duplicate removal declines (list beyond its capacity, or libstdc++ would have left quicksort)
-  auto host_filter_tail = [&]() -> int {
-    const uint32_t *h_keys = (const uint32_t *)t->h_pin;
-    const uint8_t *h_vis = t->h_pin + (size_t)std::max(nmap, 1) * 8;
-    if (nmap > 0) {
-      MVO_CUDA(ctx, cudaMemcpyAsync(t->h_pin, d_keysvis, (size_t)nmap * 9, cudaMemcpyDeviceToHost, ctx->stream));
-      MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    std::vector<MatchPair> &pairs = t->pairs;
-    int ncand = 0;
-    host_match_filter(ctx->prm, method, can_match, h_keys, h_vis, nmap, pairs, &ncand);
-    const int nm = (int)pairs.size();
-    int32_t *h_pairs = (int32_t *)(t->h_pin + al256((size_t)std::max(nmap, 1) * 9));
-    for (int i = 0; i < nm; ++i) { h_pairs[2 * i] = pairs[i].map; h_pairs[2 * i + 1] = pairs[i].train; }
-    int32_t *h_fi = h_pairs + 2 * (size_t)nm;          // filter record, same layout as the kernel writes
-    h_fi[0] = nm; h_fi[1] = ncand; h_fi[2] = 0;
-    MVO_CUDA(ctx, cudaMemcpyAsync(t->d_pairs, h_pairs, (size_t)nm * 8, cudaMemcpyHostToDevice, ctx->stream));
-    MVO_CUDA(ctx, cudaMemcpyAsync(d_finfo, h_fi, 12, cudaMemcpyHostToDevice, ctx->stream));
-    return enqueue_tail(nm, nullptr, false);
-  };
-
+  DevFrame fr;
+  MVO_TRY(frame_begin(t, fr, job, slot, ref_k));
+  int rc = frame_match(t, fr);
+  if (rc != MVO_OK) return drop_frame(t, rc);
   // The device filter restates the quicksort phase of libstdc++'s std::sort and declines when that phase would hit
   // its depth limit (libstdc++ then heapsorts: inherently sequential).  Match lists in a presorted-by-level map order
   // do that on every frame, so after a decline the next frames go straight to the host filter.
-  bool fused = nmap > 0 && !force_host_filter && t->fused_holdoff == 0;
+  bool fused = fr.nmap > 0 && fr.filter_on_device;
   if (t->fused_holdoff > 0) --t->fused_holdoff;
-  // the head of a frame's chain: match filter (in-view test, thresholds, duplicate removal, PnP input arrays) + the PnP kernels;
-  // side-effect free apart from scratch buffers.  Tcw_host / d_Tcw: the guess pose as a kernel argument or in device memory.
-  auto enqueue_head = [&](const ExtractJob &jb, int jslot, const double *Tcw_host, const double *d_Tcw, int *n_upper_out) -> int {
-    uint8_t *kv = t->d_keysvis[jslot];
-    const int n_up = std::min(nmap, std::max(jb.nk, 0));
-    MvoTrackFilter f;
-    memset(&f, 0, sizeof f);
-    f.d_keys = (uint32_t *)kv; f.d_vis = kv + (size_t)std::max(nmap, 1) * 8; f.nmap = nmap; f.nk = jb.nk; f.method = method;
-    f.d_pairs = t->d_pairs; f.d_info = d_finfo;
-    if (Tcw_host || d_Tcw) { f.Tcw12 = Tcw_host; f.d_Tcw12 = d_Tcw; f.K = t->K; f.rows = t->rows; f.cols = t->cols; }
-    f.d_map_pts = t->d_map_pts;
-    int rch = MVO_OK;
-    if (n_up >= 4) {             // the filter writes the PnP input arrays itself
-      double *d_pose_io;
-      int32_t *d_out_i, *d_inl;
-      rch = mvo_pnp_dev_buffers(ctx, n_up, &f.d_p3, &f.d_p2, &d_pose_io, &d_out_i, &d_inl);
-      f.d_kpts = jb.d_k;
-    }
-    if (rch == MVO_OK) rch = mvo_track_match_filter(ctx, f);
-    *n_upper_out = n_up;
-    return rch;
-  };
   if (fused) {
-    int n_upper = 0;
-    const bool spec_ok = t->spec.valid && t->spec.serial == job.serial && t->spec.map_version == t->map_version && ref_slot >= 0 &&
-                         t->spec.ref_slot == ref_slot && t->spec.nmap == nmap && t->spec.nk == nk && t->spec.method == method && prematched &&
-                         project_in_filter && can_match;
+    // a chain head enqueued ahead of time needs the ring pose, the pre-matched keys and the in-view test in the filter
+    const bool chain_ok = fr.ref_slot >= 0 && fr.prematched && fr.project_in_filter && fr.can_match;
+    const bool spec_ok = chain_ok && t->spec.valid && t->spec.serial == job.serial && t->spec.map_version == t->map_version &&
+                         t->spec.ref_slot == fr.ref_slot && t->spec.nmap == fr.nmap && t->spec.nk == fr.nk && t->spec.method == fr.method;
     t->spec.valid = false;
+    int n_upper = 0;
     if (spec_ok) {               // the filter and the PnP kernels of this frame are already in the stream (or done)
       n_upper = t->spec.n_upper;
-      pnp_enqueued = n_upper >= 4;
+      fr.pnp_enqueued = n_upper >= 4;
       ++t->spec_hits;
     } else {
-      rc = enqueue_head(job, slot, project_in_filter ? Tcw : nullptr, nullptr, &n_upper);
+      rc = enqueue_head(t, fr, job, fr.d_keysvis, fr.project_in_filter ? fr.Tcw : nullptr, nullptr, &n_upper);
     }
     // next frame: its extraction and pre-match run on the worker while this frame is tracked; once they are done its chain head
-    // goes into the stream behind this frame's results, with the reference pose read from the ring slot this frame's BA may move
-    if (allow_spec && ref_slot >= 0 && project_in_filter && can_match && prematched && t->n_submit != t->n_consume && rc == MVO_OK) {
-      speculate = [&, ref_slot]() -> int {
-        const int ns = (int)(t->n_consume % MVO_XSLOTS);
-        ExtractJob &nj = t->job[ns];
-        if (nj.want_host) return MVO_OK;
-        wait_job(t, ns);
-        const int mode = method == 1 ? 0 : 1;
-        if (nj.rc != MVO_OK || !nj.matched || nj.map_version != t->map_version || nj.match_mode != mode || nj.nk <= 0 || (method == 2 && nj.nk < 2))
-          return MVO_OK;
-        int n_up = 0;
-        int rcs = enqueue_head(nj, ns, nullptr, t->d_pose + (size_t)ref_slot * 12, &n_up);
-        if (rcs == MVO_OK && n_up >= 4) rcs = mvo_pnp_dev_run(ctx, n_up, t->K, d_finfo);
-        if (rcs != MVO_OK) return rcs;
-        t->spec.valid = true; t->spec.serial = nj.serial; t->spec.map_version = t->map_version; t->spec.ref_slot = ref_slot;
-        t->spec.nmap = nmap; t->spec.nk = nj.nk; t->spec.method = method; t->spec.n_upper = n_up;
-        ++t->spec_issued;
-        return MVO_OK;
-      };
-    }
-    if (rc == MVO_OK) rc = enqueue_tail(n_upper, d_finfo, true);
-    speculate = nullptr;
-    if (rc != MVO_OK) { t->spec.valid = false; return fail(rc); }
+    // goes into the stream behind this frame's results
+    if (rc == MVO_OK) rc = enqueue_tail(t, fr, n_upper, &t->d_blk->filter[FI_PAIRS], true, allow_spec && chain_ok && t->n_submit != t->n_consume);
+    if (rc != MVO_OK) { t->spec.valid = false; return drop_frame(t, rc); }
     TMARK(0);
     // the device filter declined: redo the tail through the host (its first pass saw zero pairs: only the in-view counts were taken)
-    if (h_flags[42] != 0) { fused = false; counted = true; t->fused_holdoff = 64; t->spec.valid = false; }
+    if (fr.h_blk->filter[FI_STATUS] != 0) { fused = false; fr.counted = true; t->fused_holdoff = 64; t->spec.valid = false; }
   }
   if (!fused) {
-    rc = host_filter_tail();
-    if (rc != MVO_OK) return fail(rc);
+    rc = host_filter_redo(t, fr);
+    if (rc != MVO_OK) return drop_frame(t, rc);
     TMARK(1);
   }
-
-  const int32_t *h_res_i = h_flags + 8, *h_info = h_flags + 16;
-  const double *h_res_d = (const double *)(h_out + 256), *h_stats = (const double *)(h_out + 512);
-  const double *h_ring = (const double *)(h_out + 768);
-  if (t->ring_host.size() >= (size_t)t->dev_ring * 12) memcpy(t->ring_host.data(), h_ring, (size_t)t->dev_ring * 96);
-  r.n_matches = h_flags[40];
-  r.n_candidates = h_flags[41];
-  const bool pnp_ok = h_res_i[1] != 0;
-  r.n_inliers = h_res_i[2];
-  r.pnp_ok = pnp_ok;
-  cur.n_links = h_res_i[2];
-  if (pnp_ok) Rt12_to_Twc(h_res_d, cur.T_w_c);
-  else if (t->has_prev) memcpy(cur.T_w_c, t->T_prev, sizeof cur.T_w_c);
-  memcpy(r.T_w_c_pnp, cur.T_w_c, sizeof r.T_w_c_pnp);
-  if (st.nslots > 0 && pnp_ok) {
-    const int F = h_info[0];
-    if (F < 0) { t->frames.pop_back(); return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "tracker: BA graph exceeds the device-resident kernel"); }
-    for (int f = 0; f < F; ++f) {
-      const int s = h_info[2 + f];
-      for (int b = total - 1; b >= 0; --b)
-        if (t->frames[b].slot == s) { Rt12_to_Twc(h_ring + (size_t)s * 12, t->frames[b].T_w_c); break; }
-    }
-    r.ba_frames = F;
-    r.ba_edges = h_info[1];
-    static const bool ba_dbg = getenv("MVO_BA_DEBUG") != nullptr;
-    if (ba_dbg)
-      fprintf(stderr, "k_ba_pose(store): F=%d E=%d it=%.0f trials=%.0f rejected=%.0f cycles solve=%.0f pass=%.0f gather=%.0f decide=%.0f | "
-              "pdl_wait=%.0f setup=%.0f init=%.0f exit=%.0f kernel=%.0f\n", F, h_info[1], h_stats[2], h_stats[15], h_stats[7], h_stats[8],
-              h_stats[9], h_stats[10], h_stats[11], h_stats[12], h_stats[4], h_stats[5], h_stats[6], h_stats[13]);
-  }
+  mvo_track_result r;
+  MVO_TRY(read_results(t, fr, r));
   TMARK(2);
   if (dbg && ++nacc % 50 == 0) {
+    const int32_t *fi = fr.h_blk->filter;
     fprintf(stderr, "tracker(device) us/frame: fused frame (launch .. sync) %.1f host-filter redo %.1f finish %.1f | filter kernel cycles: prologue %d sort %d (%d levels, %d segments heapsorted, longest %d) epilogue %d\n",
-            acc[0] / 50, acc[1] / 50, acc[2] / 50, h_flags[44], h_flags[45], h_flags[48], h_flags[43], h_flags[47], h_flags[46]);
+            acc[0] / 50, acc[1] / 50, acc[2] / 50, fi[FI_CYC_PROLOGUE], fi[FI_CYC_SORT], fi[FI_LEVELS], fi[FI_HEAP_SEGS], fi[FI_HEAP_MAX], fi[FI_CYC_EPILOGUE]);
     fprintf(stderr, "  chain heads enqueued ahead of time: %llu issued, %llu used\n", (unsigned long long)t->spec_issued, (unsigned long long)t->spec_hits);
     fprintf(stderr, "  per level (cycles, nbig*1000+nsmall):");
-    for (int l = 0; l < 7; ++l) fprintf(stderr, " %d/%d", h_flags[49 + 2 * l], h_flags[50 + 2 * l]);
+    for (int l = 0; l < 7; ++l) fprintf(stderr, " %d/%d", fi[FI_LEVEL + 2 * l], fi[FI_LEVEL + 2 * l + 1]);
     fprintf(stderr, "\n");
     for (double &a : acc) a = 0;
   }
 #undef TMARK
-  finish_frame(t, pnp_ok, T_w_c_out);
+  finish_frame(t, r.pnp_ok != 0, T_w_c_out);
   if (res) *res = r;
   return MVO_OK;
 }
@@ -1272,9 +1280,7 @@ static int track_host_arrays(mvo_tracker *t, ExtractJob &job, double *T_w_c_out,
 #define TMARK(i) do { if (dbg) { const double t_ = now_us(); acc[i] += t_ - t0; t0 = t_; } } while (0)
 
   // pushFrameToBuff_ (vo.h:81-86) + Frame::calcKeyPoints / calcDescriptors (done by the extraction worker)
-  t->frames.emplace_back();
-  if ((int)t->frames.size() > t->prm.buffer_size) t->frames.pop_front();
-  TrackedFrame &cur = t->frames.back();
+  TrackedFrame &cur = push_frame(t, false);
   const int nk = job.nk;
   const mvo_keypoint *kpts = job.kpts.data();
   const uint8_t *d_desc = job.d_d;
@@ -1297,15 +1303,9 @@ static int track_host_arrays(mvo_tracker *t, ExtractJob &job, double *T_w_c_out,
     uint8_t *cd = t->cand_desc.data();
     const float fcols = (float)t->cols, frows = (float)t->rows;
     for (int i = 0; i < nmap; ++i) {
-      // basics::preTranslatePoint3f: double accumulation of T(row, j) * p[j] (j = 0..3), narrowed to float
-      const double p0 = mp[3 * i], p1 = mp[3 * i + 1], p2 = mp[3 * i + 2];
-      double q[3];
-      for (int row = 0; row < 3; ++row) {
-        double acc = 0;
-        acc += Tcw[row * 4] * p0; acc += Tcw[row * 4 + 1] * p1; acc += Tcw[row * 4 + 2] * p2; acc += Tcw[row * 4 + 3] * 1.0;
-        q[row] = acc;
-      }
-      const float cx = (float)q[0], cy = (float)q[1], cz = (float)q[2];
+      float pc[3];
+      pre_translate(mp + 3 * i, Tcw, pc);
+      const float cx = pc[0], cy = pc[1], cz = pc[2];
       if (cz < 0) continue;
       // geometry::cam2pixel (camera.cpp): K(0,0) * p.x / p.z + K(0,2) in double, narrowed to Point2f
       const float u = (float)(t->K[0] * cx / cz + t->K[2]), v = (float)(t->K[4] * cy / cz + t->K[5]);
@@ -1362,8 +1362,7 @@ static int track_host_arrays(mvo_tracker *t, ExtractJob &job, double *T_w_c_out,
       }
       double Tc[16], R[9];
       rvec_to_R(rvec, R);
-      for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) Tc[i * 4 + j] = R[i * 3 + j]; Tc[i * 4 + 3] = tvec[i]; }
-      Tc[12] = Tc[13] = Tc[14] = 0; Tc[15] = 1;
+      rt_to_T(R, tvec, Tc);
       inv_rigid(Tc, cur.T_w_c);             // vo.cpp:357: T_w_c = [R|t]^-1
       // vo.cpp:360-369: reject jumps relative to the previous frame
       if (t->has_prev && trans_dist(cur.T_w_c, t->T_prev) >= t->prm.max_dist_to_prev) pnp_ok = false;

@@ -91,7 +91,6 @@ struct VoMapPoint {                                              // vo::MapPoint
   int visible_times = 1, matched_times = 1;
 };
 
-void set_identity(double *T) { memset(T, 0, 16 * sizeof(double)); T[0] = T[5] = T[10] = T[15] = 1; }
 void mul44(const double *A, const double *B, double *C) {
   double r[16];
   for (int i = 0; i < 4; ++i) for (int j = 0; j < 4; ++j) {
@@ -100,26 +99,6 @@ void mul44(const double *A, const double *B, double *C) {
     r[i * 4 + j] = a;
   }
   memcpy(C, r, sizeof r);
-}
-void inv_rigid44(const double *T, double *Ti) {                  // [R t; 0 1]^-1
-  double r[16];
-  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) r[i * 4 + j] = T[j * 4 + i];
-  for (int i = 0; i < 3; ++i) r[i * 4 + 3] = -(r[i * 4] * T[3] + r[i * 4 + 1] * T[7] + r[i * 4 + 2] * T[11]);
-  r[12] = r[13] = r[14] = 0; r[15] = 1;
-  memcpy(Ti, r, sizeof r);
-}
-void rt_to_T(const double *R, const double *t, double *T) {      // basics::convertRt2T
-  for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) T[i * 4 + j] = R[i * 3 + j]; T[i * 4 + 3] = t[i]; }
-  T[12] = T[13] = T[14] = 0; T[15] = 1;
-}
-// basics::preTranslatePoint3f: T(row, j) * p[j] accumulated in double over j = 0..3, narrowed to Point3f
-void pre_translate(const float *p, const double *T, float *out) {
-  const double p0 = p[0], p1 = p[1], p2 = p[2];
-  for (int r = 0; r < 3; ++r) {
-    double a = 0;
-    a += T[r * 4] * p0; a += T[r * 4 + 1] * p1; a += T[r * 4 + 2] * p2; a += T[r * 4 + 3] * 1.0;
-    out[r] = (float)a;
-  }
 }
 // basics::transCoord (opencv_funcs.cpp:121-125): R * p + t in double, narrowed to Point3f
 void trans_coord(const float *p, const double *R, const double *t, float *out) {
@@ -359,7 +338,7 @@ int estimate_motion_and_3d_points(mvo_vo *v, mvo_vo_frame_info *info, int *usabl
   }
   double Trt[16], Tinv[16];
   rt_to_T(R, t, Trt);
-  inv_rigid44(Trt, Tinv);
+  inv_rigid(Trt, Tinv);
   mul44(r.T_w_c, Tinv, c.T_w_c);                                 // vo.cpp:91
   MVO_TRY(retain_good_triangulation(v));
   *usable = 1;
@@ -367,7 +346,7 @@ int estimate_motion_and_3d_points(mvo_vo *v, mvo_vo_frame_info *info, int *usabl
   if (N < 20) return MVO_OK;                                     // vo.cpp:97-101
   MVO_TRY(mvo_normalize_init_depth(c.inliers_pts3d.data(), N, t, v->prm.assumed_mean_depth_init, nullptr));     // :104-108
   rt_to_T(R, t, Trt);
-  inv_rigid44(Trt, Tinv);
+  inv_rigid(Trt, Tinv);
   mul44(r.T_w_c, Tinv, c.T_w_c);                                 // :110
   return MVO_OK;
 }
@@ -437,7 +416,7 @@ bool project_in_frame(const mvo_vo *v, const double *T_c_w, const float *pos, fl
 void optimize_map(mvo_vo *v) {
   const VoFrame &c = *v->curr;
   double Tcw[16];
-  inv_rigid44(c.T_w_c, Tcw);
+  inv_rigid(c.T_w_c, Tcw);
   const double cam[3] = {c.T_w_c[3], c.T_w_c[7], c.T_w_c[11]};
   for (auto it = v->map_points.begin(); it != v->map_points.end();) {
     const VoMapPoint &mp = it->second;
@@ -467,7 +446,7 @@ int pose_estimation_pnp(mvo_vo *v, mvo_vo_frame_info *info, bool *good) {
   VoFrame &c = *v->curr;
   // getMappointsInCurrentView_ (vo.cpp:16-49): container order
   double Tcw[16];
-  inv_rigid44(c.T_w_c, Tcw);
+  inv_rigid(c.T_w_c, Tcw);
   const size_t nmap = v->map_points.size();
   v->cand_id.clear(); v->cand_xy.clear(); v->cand_desc.clear();
   v->cand_id.reserve(nmap); v->cand_xy.reserve(nmap * 2); v->cand_desc.reserve(nmap * 32);
@@ -513,10 +492,8 @@ int pose_estimation_pnp(mvo_vo *v, mvo_vo_frame_info *info, bool *good) {
       double R[9], Tc[16];
       rodrigues_to_R(rvec, R);
       rt_to_T(R, tvec, Tc);
-      inv_rigid44(Tc, c.T_w_c);                                  // vo.cpp:357
-      const double *a = c.T_w_c, *b = v->prev->T_w_c;            // vo.cpp:360-369
-      const double dx = a[3] - b[3], dy = a[7] - b[7], dz = a[11] - b[11];
-      if (sqrt(dx * dx + dy * dy + dz * dz) >= v->prm.track.max_dist_to_prev) ok = false;
+      inv_rigid(Tc, c.T_w_c);                                  // vo.cpp:357
+      if (trans_dist(c.T_w_c, v->prev->T_w_c) >= v->prm.track.max_dist_to_prev) ok = false;      // vo.cpp:360-369
     }
   }
   if (!ok) memcpy(c.T_w_c, v->prev->T_w_c, sizeof c.T_w_c);      // vo.cpp:376-379
@@ -628,7 +605,7 @@ int insert_keyframe(mvo_vo *v, mvo_vo_frame_info *info) {
   }
   // helperTriangulatePoints with the known motion getMotionFromFrame1to2(curr_, ref_) = curr^-1 * ref (vo_commons.cpp:9-15)
   double Tci[16], T[16], R[9], t[3];
-  inv_rigid44(c.T_w_c, Tci);
+  inv_rigid(c.T_w_c, Tci);
   mul44(Tci, r.T_w_c, T);
   for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) R[i * 3 + j] = T[i * 4 + j]; t[i] = T[i * 4 + 3]; }
   auto to_norm_plane = [&](const mvo_dmatch &m, float *a, float *b) {        // pixel2CamNormPlane (camera.cpp:10-15)
@@ -879,9 +856,8 @@ int mvo_vo_add_frame_ex(mvo_vo *v, const uint8_t *image, int channels, size_t st
       if (v->buff[v->buff.size() - 1 - (size_t)k] == v->ref) { ref_k = k; break; }
     int allow_spec = 0;
     {
-      auto dist = [](const double *A, const double *B) { const double dx = A[3] - B[3], dy = A[7] - B[7], dz = A[11] - B[11]; return sqrt(dx * dx + dy * dy + dz * dz); };
-      const double d_prev = dist(v->prev->T_w_c, v->ref->T_w_c);
-      const double step = v->buff.size() >= 3 ? dist(v->prev->T_w_c, v->buff[v->buff.size() - 3]->T_w_c) : 0.0;
+      const double d_prev = trans_dist(v->prev->T_w_c, v->ref->T_w_c);
+      const double step = v->buff.size() >= 3 ? trans_dist(v->prev->T_w_c, v->buff[v->buff.size() - 3]->T_w_c) : 0.0;
       allow_spec = d_prev + 1.1 * step < v->prm.track.min_dist_keyframe;
     }
     rc = mvo_trk_track(v->trk, slot, v->ref->T_w_c, v->prev->T_w_c, frame->T_w_c, &r, ref_k, allow_spec);
