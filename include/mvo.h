@@ -433,6 +433,39 @@ typedef struct mvo_two_view_solutions {
 int mvo_estimate_relative_poses(mvo_ctx *ctx, const float *pts_img1, const float *pts_img2, int n, const double *K,
                                 int calc_homo, int motion_cam2_to_cam1, mvo_two_view_solutions *sol,
                                 int32_t *inliers, float *pts3d);
+/* helperEstimatePossibleRelativePosesByEpipolarGeometry with the homography branch (what the reference's callers use:
+ * vo.cpp:65-75, test_epipolor_geometry.cpp:105-113) for the matched frame pairs of a batch, entirely on the device: pair p gets
+ * what mvo_estimate_relative_poses(calc_homo = 1, motion_cam2_to_cam1) returns for its points.
+ * d_kpts / d_counts / batch / cap / d_pairs / d_matches / d_n_matches: as for mvo_esti_motion_by_essential_batch_dev (same
+ * layouts, same per-pair input checks); pair p's correspondences are kpts[query frame][m.query_idx].pt <->
+ * kpts[train frame][m.train_idx].pt in match-list order.  K: host 3x3.  The thresholds are those of a single call:
+ * mvo_params::essential_threshold, homography_threshold, eh_ratio_threshold, epi_hypotheses and pnp_seed.
+ * d_res[p]: status MVO_OK or the mvo_status of that pair alone, n_matches = d_n_matches[p] as given, and on MVO_OK `sol`
+ * byte-identical to what mvo_estimate_relative_poses writes (every byte: unused solution slots, normal[0] and pad_ are 0; H and
+ * score_h are 0 when the homography RANSAC found no model).  A failed pair writes its status and n_matches only (not the rest
+ * of its record, its inlier rows or its points):
+ *   MVO_ERR_INVALID_ARG  a frame index outside [0, batch), a match count outside [0, cap], a keypoint index outside its frame;
+ *   MVO_ERR_DEGENERATE   fewer than 8 matches, or no essential matrix reaches 8 inliers.
+ * A homography that reaches fewer than 4 inliers is not a failure: num_solutions = 1, as in the single call.
+ * Solution s of pair p: its n_inliers[s] inlier indices at d_inliers + (p * 5 + s) * cap (row 0 the essential inliers, rows
+ * 1..num_solutions-1 the homography inliers), its triangulated inliers at d_pts3d + (p * 5 + s) * cap * 3 (d_pts3d NULL: no
+ * triangulation); rows past num_solutions are not written.
+ * NaN: ratio = score_h / (score_e + score_h) is 0 / 0 when both scores are 0.  The single call computes it on x86-64, whose
+ * default NaN is 0xFFF8000000000000; the device writes that bit pattern for a NaN score_e, score_h or ratio, so such a pair
+ * is byte-identical too (points with NaN coordinates, whose payloads the host would propagate, are outside this promise).
+ * MVO_ERR_INVALID_ARG: a null pointer, fx or fy <= 0, a singular K.  MVO_ERR_UNSUPPORTED: cap > 6400, n_pairs > 65535,
+ * n_pairs x epi_hypotheses > 2^22 (80 bytes of scratch per hypothesis, shared by the essential and the homography half).
+ * Asynchronous on the context stream: ten kernel launches (eleven with d_pts3d) whatever n_pairs is, no host synchronisation
+ * except when the call's own scratch buffer of the context has to grow. */
+typedef struct mvo_relative_poses_result {
+  int32_t status;              /* MVO_OK, or the mvo_status the per-pair call would have returned */
+  int32_t n_matches;           /* the pair's match count, d_n_matches[p] */
+  mvo_two_view_solutions sol;  /* byte-identical to what mvo_estimate_relative_poses writes */
+} mvo_relative_poses_result;
+int mvo_estimate_relative_poses_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                          const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
+                                          const int32_t *d_n_matches, const double *K, int motion_cam2_to_cam1,
+                                          mvo_relative_poses_result *d_res, int32_t *d_inliers, float *d_pts3d);
 
 /* ---- host-side decisions of the initialisation / keyframe logic (SURVEY.md 8f-2; no context, no GPU) ----------
  * retainGoodTriangulationResult_ (src/vo/vo.cpp:181-244): triangulation angle (degrees, with the reference's

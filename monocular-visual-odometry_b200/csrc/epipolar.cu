@@ -22,6 +22,7 @@
 #include <string.h>
 #include <vector>
 #include "epipolar_math.cuh"
+#include "eh_scores.cuh"
 #include "mvo_internal.h"
 
 namespace {
@@ -135,6 +136,65 @@ int mvo_epi_essential_ex(mvo_ctx *ctx, const float *pts1, const float *pts2, int
   return mvo_epi_essential_end(ctx, &job, E, R, t, inliers, n_inliers, tri_out);
 }
 
+namespace {
+
+// the call-level checks of both batch calls (mvo.h)
+int epi_batch_check(mvo_ctx *ctx, const char *what, int batch, int cap, int n_pairs, const double *K) {
+  if (n_pairs < 0 || batch < 1 || cap < 1) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "%s: n_pairs=%d batch=%d cap=%d", what, n_pairs, batch, cap);
+  if (!(K[0] > 0 && K[4] > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal lengths must be positive");
+  if ((size_t)cap * 4 * sizeof(double) > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "%s: cap %d above %d correspondences", what, cap, 200 * 1024 / 32);
+  if (n_pairs > 65535) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "%s: %d pairs, at most 65535 per call", what, n_pairs);
+  const int H = ctx->prm.epi_hypotheses;
+  if ((size_t)n_pairs * H > ((size_t)1 << 22)) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "%s: %d pairs x %d hypotheses above 2^22 per call", what, n_pairs, H);
+  return MVO_OK;
+}
+
+// Scratch of the essential half: gathered points (np1 / np2 optional), pn, hypothesis rows (Es 72 B + valid 4 B + cnt 4 B per
+// hypothesis), finish outputs
+struct EpiBatchScratch {
+  float *p1, *p2, *np1, *np2;
+  int32_t *pn, *valid, *cnt, *oi;
+  double *Es, *od;
+};
+
+// gather, hypotheses, scoring, finish, vote, pick: six launches; pair p's inliers at inl + p * cap, its record in res[p]
+int epi_essential_batch_enqueue(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap, const int32_t *d_pairs,
+                                int n_pairs, const mvo_dmatch *d_matches, const int32_t *d_n_matches, const double *K, double threshold,
+                                const EpiBatchScratch &b, mvo_two_view_result *res, int32_t *inl) {
+  EpiCam cam;
+  cam.f = (K[0] + K[4]) / 2; cam.cx = K[2]; cam.cy = K[5];
+  const int H = ctx->prm.epi_hypotheses;
+  const size_t smem = (size_t)cap * 4 * sizeof(double);
+  const double thr2 = (threshold / cam.f) * (threshold / cam.f);          // as mvo_epi_essential_begin
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_gather<<<n_pairs, 256, 0, ctx->stream>>>(d_kpts, d_counts, batch, cap, (const int2 *)d_pairs, d_matches, d_n_matches, K[0], K[4], K[2], K[5],
+                                                 b.p1, b.p2, b.np1, b.np2, b.pn); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_hypotheses_batch<<<dim3((H + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(b.p1, b.p2, b.pn, cap, cam, ctx->prm.pnp_seed, H, b.Es, b.valid); }
+  MVO_CHECK_LAUNCH(ctx);
+  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_epi_score_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // about as many CTAs in all as the single call uses for its one pair, at least one per pair
+  int per_pair = (4 * ctx->sm_count + n_pairs - 1) / n_pairs;
+  if (per_pair > (H + 7) / 8) per_pair = (H + 7) / 8;
+  { KTimer kt(ctx, KC_EPI_SCORE);
+  k_epi_score_batch<<<dim3(per_pair, n_pairs), 256, smem, ctx->stream>>>(b.p1, b.p2, b.pn, cap, cam, thr2, H, b.Es, b.valid, b.cnt); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI_FINISH);
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(EpiFinSmem), k_epi_finish_batch, (const float *)b.p1, (const float *)b.p2,
+                                        (const int32_t *)b.pn, cap, cam, thr2, H, (const double *)b.Es, (const int32_t *)b.cnt, b.od, b.oi, inl)); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_vote_batch<<<dim3((cap + 63) / 64, n_pairs), 256, 0, ctx->stream>>>(b.p1, b.p2, b.pn, cap, cam, b.od, b.oi, inl); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_pick<<<(n_pairs + 127) / 128, 128, 0, ctx->stream>>>(b.pn, n_pairs, b.od, b.oi, res); }
+  MVO_CHECK_LAUNCH(ctx);
+  return MVO_OK;
+}
+
+}  // namespace
+
 // mvo_esti_motion_by_essential_batch_dev (mvo.h): gather, hypotheses, scoring, finish, vote, pick (+ triangulation) for every
 // pair at once; the scratch lives in ctx->epib_buf
 extern "C" int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
@@ -144,19 +204,10 @@ extern "C" int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_ke
   if (!ctx) return MVO_ERR_INVALID_ARG;
   if (!d_kpts || !d_counts || !d_pairs || !d_matches || !d_n_matches || !K || !d_res || !d_inliers)
     return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: null pointer");
-  if (n_pairs < 0 || batch < 1 || cap < 1)
-    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: n_pairs=%d batch=%d cap=%d", n_pairs, batch, cap);
-  if (!(K[0] > 0 && K[4] > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal lengths must be positive");
   if (!(threshold > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: threshold must be positive");
-  const size_t smem = (size_t)cap * 4 * sizeof(double);
-  if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential batch: cap %d above %d correspondences", cap, 200 * 1024 / 32);
-  if (n_pairs > 65535) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential batch: %d pairs, at most 65535 per call", n_pairs);
-  const int H = ctx->prm.epi_hypotheses;
-  if ((size_t)n_pairs * H > ((size_t)1 << 22))
-    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential batch: %d pairs x %d hypotheses above 2^22 per call", n_pairs, H);
+  MVO_TRY(epi_batch_check(ctx, "estiMotionByEssential batch", batch, cap, n_pairs, K));
   if (n_pairs == 0) return MVO_OK;
-  EpiCam cam;
-  cam.f = (K[0] + K[4]) / 2; cam.cx = K[2]; cam.cy = K[5];
+  const int H = ctx->prm.epi_hypotheses;
   const bool tri = d_pts3d != nullptr;
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
   auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
@@ -166,37 +217,93 @@ extern "C" int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_ke
   const size_t o_oi = al(o_od + np * EPIB_OUT_D * 8), o_end = o_oi + np * EPIB_OUT_I * 4;
   MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, o_end));
   uint8_t *d = (uint8_t *)ctx->epib_buf.p;
-  float *p1 = (float *)(d + o_p1), *p2 = (float *)(d + o_p2), *np1 = tri ? (float *)(d + o_n1) : nullptr, *np2 = tri ? (float *)(d + o_n2) : nullptr;
-  int32_t *pn = (int32_t *)(d + o_pn), *valid = (int32_t *)(d + o_valid), *cnt = (int32_t *)(d + o_cnt), *oi = (int32_t *)(d + o_oi);
-  double *Es = (double *)(d + o_E), *od = (double *)(d + o_od);
-  const double thr2 = (threshold / cam.f) * (threshold / cam.f);          // as mvo_epi_essential_begin
+  EpiBatchScratch b;
+  b.p1 = (float *)(d + o_p1); b.p2 = (float *)(d + o_p2); b.np1 = tri ? (float *)(d + o_n1) : nullptr; b.np2 = tri ? (float *)(d + o_n2) : nullptr;
+  b.pn = (int32_t *)(d + o_pn); b.valid = (int32_t *)(d + o_valid); b.cnt = (int32_t *)(d + o_cnt); b.oi = (int32_t *)(d + o_oi);
+  b.Es = (double *)(d + o_E); b.od = (double *)(d + o_od);
+  MVO_TRY(epi_essential_batch_enqueue(ctx, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K, threshold, b, d_res, d_inliers));
+  if (tri) {
+    KTimer kt(ctx, KC_EPI);
+    k_triangulate_batch<<<dim3((cap + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(b.np1, b.np2, d_res, cap, d_inliers, d_pts3d);
+    MVO_CHECK_LAUNCH(ctx);
+  }
+  return MVO_OK;
+}
+
+// The combine step lives in two_view_batch.cu, a translation unit of its own that is compiled without contraction (Makefile).
+// libmvo.so always links it; a library assembled from a subset of the units without it reports MVO_ERR_UNSUPPORTED for the call.
+int mvo_relative_poses_combine(mvo_ctx *ctx, const MvoRelPosesCombine &a) __attribute__((weak));
+
+// mvo_estimate_relative_poses_batch_dev (mvo.h): the essential half (six launches, into an internal mvo_two_view_result array),
+// the homography half (three launches), the combine step (two_view_batch.cu: decomposition, visibility filter, inlier rows,
+// invRt, scores, E/H choice) and, with d_pts3d, one triangulation launch over (pair, solution).  Scratch in ctx->epib_buf: the
+// homography half reuses the essential half's hypothesis rows (80 B per hypothesis), which k_epi_finish_batch has consumed by the
+// time k_homo_hypotheses_batch runs on the same stream.
+extern "C" int mvo_estimate_relative_poses_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                                     const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
+                                                     const int32_t *d_n_matches, const double *K, int motion_cam2_to_cam1,
+                                                     mvo_relative_poses_result *d_res, int32_t *d_inliers, float *d_pts3d) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (!d_kpts || !d_counts || !d_pairs || !d_matches || !d_n_matches || !K || !d_res || !d_inliers)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estimate_relative_poses batch: null pointer");
+  if (!mvo_relative_poses_combine)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estimate_relative_poses batch: the library was built without two_view_batch.cu");
+  MVO_TRY(epi_batch_check(ctx, "estimate_relative_poses batch", batch, cap, n_pairs, K));
+  double Ki[9];
+  if (!epi::inv3(K, Ki)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: singular (checkEssentialScore inverts it)");
+  if (n_pairs == 0) return MVO_OK;
+  const int H = ctx->prm.epi_hypotheses;
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t np = (size_t)n_pairs, pts = al(np * cap * 8), idx = al(np * cap * 4);
+  const size_t o_p1 = 0, o_p2 = o_p1 + pts, o_n1 = o_p2 + pts, o_n2 = o_n1 + pts, o_pn = o_n2 + pts;
+  const size_t o_E = al(o_pn + np * 4), o_valid = al(o_E + np * H * 72), o_cnt = al(o_valid + np * H * 4), o_od = al(o_cnt + np * H * 4);
+  const size_t o_oi = al(o_od + np * EPIB_OUT_D * 8), o_hd = al(o_oi + np * EPIB_OUT_I * 4), o_hi = al(o_hd + np * EPIB_OUT_D * 8);
+  const size_t o_ess = al(o_hi + np * EPIB_OUT_I * 4), o_ie = al(o_ess + np * sizeof(mvo_two_view_result)), o_ih = o_ie + idx;
+  const size_t o_rt = o_ih + idx, o_end = o_rt + np * 5 * 12 * 8;
+  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, o_end));
+  uint8_t *d = (uint8_t *)ctx->epib_buf.p;
+  EpiBatchScratch b;
+  b.p1 = (float *)(d + o_p1); b.p2 = (float *)(d + o_p2); b.np1 = (float *)(d + o_n1); b.np2 = (float *)(d + o_n2);
+  b.pn = (int32_t *)(d + o_pn); b.valid = (int32_t *)(d + o_valid); b.cnt = (int32_t *)(d + o_cnt); b.oi = (int32_t *)(d + o_oi);
+  b.Es = (double *)(d + o_E); b.od = (double *)(d + o_od);
+  mvo_two_view_result *ess = (mvo_two_view_result *)(d + o_ess);
+  int32_t *inl_e = (int32_t *)(d + o_ie), *inl_h = (int32_t *)(d + o_ih), *hoi = (int32_t *)(d + o_hi);
+  double *hod = (double *)(d + o_hd), *rt = (double *)(d + o_rt);
+  // ---- essential half (:43-48) ----
+  MVO_TRY(epi_essential_batch_enqueue(ctx, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K, ctx->prm.essential_threshold,
+                                      b, ess, inl_e));
+  // ---- homography half (:56-67), as mvo_epi_homography_begin on the same points ----
+  HomoCam hc;
+  hc.f = (K[0] + K[4]) / 2; hc.cx = K[2]; hc.cy = K[5];
+  const double hthr2 = (ctx->prm.homography_threshold / hc.f) * (ctx->prm.homography_threshold / hc.f);
+  const size_t smem = (size_t)cap * 4 * sizeof(double);
   { KTimer kt(ctx, KC_EPI);
-  k_epi_gather<<<n_pairs, 256, 0, ctx->stream>>>(d_kpts, d_counts, batch, cap, (const int2 *)d_pairs, d_matches, d_n_matches, K[0], K[4], K[2], K[5],
-                                                 p1, p2, np1, np2, pn); }
+  k_homo_hypotheses_batch<<<dim3((H + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(b.p1, b.p2, b.pn, cap, hc, ctx->prm.pnp_seed, H, b.Es, b.valid, hod, hoi); }
   MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI);
-  k_epi_hypotheses_batch<<<dim3((H + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(p1, p2, pn, cap, cam, ctx->prm.pnp_seed, H, Es, valid); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_epi_score_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  // about as many CTAs in all as the single call uses for its one pair, at least one per pair
+  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_homo_score_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_pair = (4 * ctx->sm_count + n_pairs - 1) / n_pairs;
   if (per_pair > (H + 7) / 8) per_pair = (H + 7) / 8;
   { KTimer kt(ctx, KC_EPI_SCORE);
-  k_epi_score_batch<<<dim3(per_pair, n_pairs), 256, smem, ctx->stream>>>(p1, p2, pn, cap, cam, thr2, H, Es, valid, cnt); }
+  k_homo_score_batch<<<dim3(per_pair, n_pairs), 256, smem, ctx->stream>>>(b.p1, b.p2, b.pn, cap, hc, hthr2, H, b.Es, b.valid, b.cnt); }
   MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(EpiFinSmem), k_epi_finish_batch, (const float *)p1, (const float *)p2,
-                                        (const int32_t *)pn, cap, cam, thr2, H, (const double *)Es, (const int32_t *)cnt, od, oi, d_inliers)); }
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(HomoFinSmem), k_homo_finish_batch, (const float *)b.p1, (const float *)b.p2,
+                                        (const int32_t *)b.pn, cap, hc, hthr2, H, (const double *)b.Es, (const int32_t *)b.cnt, hod, hoi, inl_h)); }
   MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI);
-  k_epi_vote_batch<<<dim3((cap + 63) / 64, n_pairs), 256, 0, ctx->stream>>>(p1, p2, pn, cap, cam, od, oi, d_inliers); }
-  MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI);
-  k_epi_pick<<<(n_pairs + 127) / 128, 128, 0, ctx->stream>>>(pn, n_pairs, od, oi, d_res); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (tri) {
+  // ---- combine (:56-154 after the RANSACs) ----
+  MvoRelPosesCombine a;
+  a.n_matches = d_n_matches; a.ess = ess; a.inl_e = inl_e; a.hom_i = hoi; a.inl_h = inl_h; a.hom_d = hod;
+  a.p1 = b.p1; a.p2 = b.p2; a.np1 = b.np1; a.np2 = b.np2;
+  a.n_pairs = n_pairs; a.cap = cap; a.hom_d_stride = EPIB_OUT_D; a.hom_i_stride = EPIB_OUT_I; a.motion_cam2_to_cam1 = motion_cam2_to_cam1;
+  for (int q = 0; q < 9; ++q) a.K[q] = K[q];
+  a.eh_ratio_threshold = ctx->prm.eh_ratio_threshold;
+  a.res = d_res; a.inliers = d_inliers; a.rt = rt;
+  MVO_TRY(mvo_relative_poses_combine(ctx, a));
+  // ---- triangulation of every solution (:105-112), with the (R, t) from before invRt ----
+  if (d_pts3d) {
     KTimer kt(ctx, KC_EPI);
-    k_triangulate_batch<<<dim3((cap + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(np1, np2, d_res, cap, d_inliers, d_pts3d);
+    k_triangulate_solutions_batch<<<dim3((cap + 127) / 128, 5, n_pairs), 128, 0, ctx->stream>>>(b.np1, b.np2, d_res, rt, cap, d_inliers, d_pts3d);
     MVO_CHECK_LAUNCH(ctx);
   }
   return MVO_OK;

@@ -618,14 +618,13 @@ k_triangulate_batch(const float *__restrict__ np1, const float *__restrict__ np2
 // (OpenCV refines its RANSAC result with LM on the same cost).  All three kernels work in isotropically scaled pixel
 // coordinates ((u - cx) / f, (v - cy) / f, f = mean focal length): errors scale by 1 / f, the conditioning of the
 // 4-point systems and of the normal equations does not depend on the image size.  The decomposition itself is a few
-// hundred flops and runs on the host (the same epipolar_math.cuh routine).
+// hundred flops and runs on the host (the same epipolar_math.cuh routine); for a batch of pairs it runs in the combine kernel of
+// two_view_batch.cu, compiled without contraction like the host code.
 struct HomoCam { double f, cx, cy; };
 
-__global__ void __launch_bounds__(128)
-k_homo_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, uint64_t seed, int H,
-                  double *__restrict__ Hs, int32_t *__restrict__ valid) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= H) return;
+// hypothesis h: counter-based minimal sample of 4 distinct correspondences, epi::homography_from_4
+__device__ __forceinline__ void homo_hypothesis(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, uint64_t seed,
+                                                int h, double *__restrict__ Hs, int32_t *__restrict__ valid) {
   int idx[4];
   uint64_t ctr = 0;
   for (int k = 0; k < 4; ++k)
@@ -649,9 +648,18 @@ k_homo_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, in
   valid[h] = ok ? 1 : 0;
 }
 
-__global__ void __launch_bounds__(256)
-k_homo_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
-             const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
+__global__ void __launch_bounds__(128)
+k_homo_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, uint64_t seed, int H,
+                  double *__restrict__ Hs, int32_t *__restrict__ valid) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= H) return;
+  homo_hypothesis(p1, p2, n, cam, seed, h, Hs, valid);
+}
+
+// forward transfer error consensus of hypotheses cta * warps + warp, strided by ncta * warps; the CTA stages the n points once
+__device__ __forceinline__ void homo_score_run(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
+                                               const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts,
+                                               int cta, int ncta) {
   EPI_DYN_SMEM(double, s_pt);         // [n][4] scaled coordinates x1 y1 x2 y2
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     s_pt[4 * i] = ((double)p1[2 * i] - cam.cx) / cam.f; s_pt[4 * i + 1] = ((double)p1[2 * i + 1] - cam.cy) / cam.f;
@@ -659,7 +667,7 @@ k_homo_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, 
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  for (int h = blockIdx.x * wpb + warp; h < H; h += gridDim.x * wpb) {
+  for (int h = cta * wpb + warp; h < H; h += ncta * wpb) {
     if (valid[h] <= 0) { if (lane == 0) counts[h] = -1; continue; }
     double Hm[9];
     for (int q = 0; q < 9; ++q) Hm[q] = Hs[(size_t)h * 9 + q];
@@ -669,6 +677,12 @@ k_homo_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, 
     for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
     if (lane == 0) counts[h] = c;
   }
+}
+
+__global__ void __launch_bounds__(256)
+k_homo_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
+             const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
+  homo_score_run(p1, p2, n, cam, thr2, H, Hs, valid, counts, blockIdx.x, gridDim.x);
 }
 
 constexpr int HOMO_NV = epi::HOMO_GN_NV;    // 45 entries of J^T J (upper triangle) + 9 of J^T r
@@ -752,10 +766,9 @@ struct HomoFinSmem {
   int cnt[EFIN_T / 32], best, stop, ipart[4];
 };
 
-__global__ void __launch_bounds__(EFIN_T, 1)
-k_homo_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
-              const double *__restrict__ Hs, const int32_t *__restrict__ counts, double *__restrict__ out_d,
-              int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
+__device__ __forceinline__ void homo_finish_run(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
+                                                const double *__restrict__ Hs, const int32_t *__restrict__ counts, double *__restrict__ out_d,
+                                                int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
   EPI_DYN_SMEM(double, smraw);
   HomoFinSmem &S = *reinterpret_cast<HomoFinSmem *>(smraw);
   cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
@@ -901,3 +914,64 @@ k_homo_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n,
   cluster.sync();                                    // no CTA leaves while another still reads its shared memory
 }
 
+__global__ void __launch_bounds__(EFIN_T, 1)
+k_homo_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
+              const double *__restrict__ Hs, const int32_t *__restrict__ counts, double *__restrict__ out_d,
+              int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
+  homo_finish_run(p1, p2, n, cam, thr2, H, Hs, counts, out_d, out_i, inl);
+}
+
+// ------------------------------------------------------------------------- homography for a batch of frame pairs
+// mvo_estimate_relative_poses_batch_dev: the three homography kernels over the pairs of the essential batch (same pn, same
+// point rows; the hypotheses reuse the essential half's hypothesis rows, which are free once k_epi_finish_batch has run).
+// Pair p's finish outputs at p * EPIB_OUT_D / p * EPIB_OUT_I: the single call zeroes its 512-byte output block before the
+// launches, k_homo_hypotheses_batch does it here (CTA 0 of each pair), so a pair without any model reads 0 inliers.
+__global__ void __launch_bounds__(128)
+k_homo_hypotheses_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, HomoCam cam,
+                        uint64_t seed, int H, double *__restrict__ Hs, int32_t *__restrict__ valid, double *__restrict__ out_d,
+                        int32_t *__restrict__ out_i) {
+  const int pair = blockIdx.y, h = blockIdx.x * blockDim.x + threadIdx.x, n = pn[pair];
+  if (blockIdx.x == 0 && threadIdx.x < EPIB_OUT_D) {
+    out_d[(size_t)pair * EPIB_OUT_D + threadIdx.x] = 0.0;
+    if (threadIdx.x < EPIB_OUT_I) out_i[(size_t)pair * EPIB_OUT_I + threadIdx.x] = 0;
+  }
+  if (h >= H || n < 8) return;
+  homo_hypothesis(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, seed, h, Hs + (size_t)pair * H * 9, valid + (size_t)pair * H);
+}
+
+// gridDim.x CTAs per pair (blockIdx.y), sized as k_epi_score_batch
+__global__ void __launch_bounds__(256)
+k_homo_score_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, HomoCam cam, double thr2,
+                   int H, const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
+  const int pair = blockIdx.y, n = pn[pair];
+  if (n < 8) return;
+  const size_t oh = (size_t)pair * H;
+  homo_score_run(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, thr2, H, Hs + oh * 9, valid + oh, counts + oh, blockIdx.x, gridDim.x);
+}
+
+// one EFIN_C-CTA cluster per pair, as k_epi_finish_batch
+__global__ void __launch_bounds__(EFIN_T, 1)
+k_homo_finish_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, HomoCam cam, double thr2,
+                    int H, const double *__restrict__ Hs, const int32_t *__restrict__ counts, double *__restrict__ out_d,
+                    int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
+  const int pair = blockIdx.x / cooperative_groups::this_cluster().num_blocks(), n = pn[pair];
+  if (n < 8) return;                                 // the whole cluster
+  const size_t op = (size_t)pair * cap, oh = (size_t)pair * H;
+  homo_finish_run(p1 + op * 2, p2 + op * 2, n, cam, thr2, H, Hs + oh * 9, counts + oh, out_d + (size_t)pair * EPIB_OUT_D,
+                  out_i + (size_t)pair * EPIB_OUT_I, inl + op);
+}
+
+// doTriangulation of solution s (blockIdx.y) of pair blockIdx.z, with the (R, t) the combine step kept from before basics::invRt
+// (mvo_estimate_relative_poses triangulates first and inverts afterwards): rt[(pair * 5 + s) * 12] = R | t, inlier row
+// (pair * 5 + s) * cap of the caller's array
+__global__ void __launch_bounds__(128)
+k_triangulate_solutions_batch(const float *__restrict__ np1, const float *__restrict__ np2, const mvo_relative_poses_result *__restrict__ res,
+                              const double *__restrict__ rt, int cap, const int32_t *__restrict__ inl, float *__restrict__ out) {
+  const int pair = blockIdx.z, s = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  const mvo_relative_poses_result &r = res[pair];
+  if (r.status != MVO_OK || s >= r.sol.num_solutions || j >= r.sol.n_inliers[s]) return;
+  double Rt[12];
+  for (int q = 0; q < 12; ++q) Rt[q] = rt[((size_t)pair * 5 + s) * 12 + q];
+  const size_t op = (size_t)pair * cap, orow = ((size_t)pair * 5 + s) * cap;
+  epi_triangulate_one(np1 + op * 2, np2 + op * 2, inl[orow + j], Rt, out + orow * 3, j);
+}

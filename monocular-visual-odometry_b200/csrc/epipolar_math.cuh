@@ -17,8 +17,9 @@
 // the three routines with nested loops over local arrays are real calls on the device: inlining them into each other
 // (essential_from_8 -> null_vector_8x9 / svd3 -> sym_eigen_jacobi) bloats every caller and, with nvcc 12.9, once
 // produced wrong singular values inside essential_from_8 although each routine is correct on its own
-// (tests/test_epipolar_gpu.py::test_device_math_equals_host_build)
-#define EPI_HD_CALL __host__ __device__ __noinline__
+// (tests/test_epipolar_gpu.py::test_device_math_equals_host_build).  `inline` for the linkage only: more than one translation
+// unit includes this header (epipolar.cu, two_view_batch.cu)
+#define EPI_HD_CALL __host__ __device__ __noinline__ inline
 #else
 #define EPI_HD inline
 #define EPI_HD_CALL inline

@@ -7,27 +7,8 @@
 #include <math.h>
 #include <stdint.h>
 #include <vector>
+#include "eh_scores.cuh"
 #include "mvo.h"
-
-namespace {
-
-bool inv3(const double *M, double *I) {
-  const double c0 = M[4] * M[8] - M[5] * M[7], c1 = M[5] * M[6] - M[3] * M[8], c2 = M[3] * M[7] - M[4] * M[6];
-  const double det = M[0] * c0 + M[1] * c1 + M[2] * c2;
-  if (!(fabs(det) > 0)) return false;
-  const double id = 1.0 / det;
-  I[0] = c0 * id; I[1] = (M[2] * M[7] - M[1] * M[8]) * id; I[2] = (M[1] * M[5] - M[2] * M[4]) * id;
-  I[3] = c1 * id; I[4] = (M[0] * M[8] - M[2] * M[6]) * id; I[5] = (M[2] * M[3] - M[0] * M[5]) * id;
-  I[6] = c2 * id; I[7] = (M[1] * M[6] - M[0] * M[7]) * id; I[8] = (M[0] * M[4] - M[1] * M[3]) * id;
-  return true;
-}
-
-void mul3(const double *A, const double *B, double *C) {
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) C[i * 3 + j] = A[i * 3] * B[j] + A[i * 3 + 1] * B[3 + j] + A[i * 3 + 2] * B[6 + j];
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -35,29 +16,20 @@ int mvo_check_essential_score(const double *E21, const double *K, const float *p
                               int32_t *inliers, int *n_inliers, double sigma, double *score_out) {
   if (!E21 || !K || !n_inliers || *n_inliers < 0 || !score_out || (*n_inliers > 0 && (!inliers || !pts_img1 || !pts_img2)) || !(sigma > 0))
     return MVO_ERR_INVALID_ARG;
-  double Ki[9], KiT[9], T[9], F[9];
-  if (!inv3(K, Ki)) return MVO_ERR_INVALID_ARG;
-  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) KiT[i * 3 + j] = Ki[j * 3 + i];
-  mul3(E21, Ki, T);
-  mul3(KiT, T, F);                                   // F21 = K^-T E21 K^-1 (:507-509)
-  const double th = 3.841, thScore = 5.991, invSigmaSquare = 1.0 / (sigma * sigma);     // :524-527
+  double Ki[9], F[9];
+  if (!epi::inv3(K, Ki)) return MVO_ERR_INVALID_ARG;
+  epi::essential_score_F(E21, Ki, F);                // F21 = K^-T E21 K^-1 (:507-509)
+  const double th = epi::EH_ESSENTIAL_TH, thScore = epi::EH_ESSENTIAL_TH_SCORE, invSigmaSquare = 1.0 / (sigma * sigma);     // :524-527
   double score = 0;
   int w = 0;
   for (int k = 0; k < *n_inliers; ++k) {
     const int i = inliers[k];
     if (i < 0 || i >= n) return MVO_ERR_INVALID_ARG;
     bool good = true;
-    const double u1 = pts_img1[2 * i], v1 = pts_img1[2 * i + 1], u2 = pts_img2[2 * i], v2 = pts_img2[2 * i + 1];
-    // distance of x2 to the epipolar line l2 = F21 x1 (:543-557)
-    const double a2 = F[0] * u1 + F[1] * v1 + F[2], b2 = F[3] * u1 + F[4] * v1 + F[5], c2 = F[6] * u1 + F[7] * v1 + F[8];
-    const double num2 = a2 * u2 + b2 * v2 + c2;
-    const double chi1 = num2 * num2 / (a2 * a2 + b2 * b2) * invSigmaSquare;
+    double chi1, chi2;                               // x2 against l2 = F21 x1, x1 against l1 = x2^T F21 (:543-573)
+    epi::essential_score_chi(F, pts_img1[2 * i], pts_img1[2 * i + 1], pts_img2[2 * i], pts_img2[2 * i + 1], invSigmaSquare, &chi1, &chi2);
     if (chi1 > th) good = false;
     else score += thScore - chi1;
-    // distance of x1 to l1 = x2^T F21 (:559-573)
-    const double a1 = F[0] * u2 + F[3] * v2 + F[6], b1 = F[1] * u2 + F[4] * v2 + F[7], c1 = F[2] * u2 + F[5] * v2 + F[8];
-    const double num1 = a1 * u1 + b1 * v1 + c1;
-    const double chi2 = num1 * num1 / (a1 * a1 + b1 * b1) * invSigmaSquare;
     if (chi2 > th) good = false;
     else score += thScore - chi2;
     if (good) inliers[w++] = i;                      // :575-576 (w <= k: in place)
@@ -72,25 +44,18 @@ int mvo_check_homography_score(const double *H21, const float *pts_img1, const f
   if (!H21 || !n_inliers || *n_inliers < 0 || !score_out || (*n_inliers > 0 && (!inliers || !pts_img1 || !pts_img2)) || !(sigma > 0))
     return MVO_ERR_INVALID_ARG;
   double H12[9];
-  if (!inv3(H21, H12)) return MVO_ERR_INVALID_ARG;
-  const double th = 5.991, invSigmaSquare = 1.0 / (sigma * sigma);       // :613-614
+  if (!epi::inv3(H21, H12)) return MVO_ERR_INVALID_ARG;
+  const double th = epi::EH_HOMOGRAPHY_TH, invSigmaSquare = 1.0 / (sigma * sigma);       // :613-614
   double score = 0;          // the reference leaves `score` uninitialised (:586); zero is what the sum is meant to start from
   int w = 0;
   for (int k = 0; k < *n_inliers; ++k) {
     const int i = inliers[k];
     if (i < 0 || i >= n) return MVO_ERR_INVALID_ARG;
     bool good = true;
-    const double u1 = pts_img1[2 * i], v1 = pts_img1[2 * i + 1], u2 = pts_img2[2 * i], v2 = pts_img2[2 * i + 1];
-    // x2 in image 1 through H12 (:628-640)
-    const double wi = 1.0 / (H12[6] * u2 + H12[7] * v2 + H12[8]);
-    const double u2in1 = (H12[0] * u2 + H12[1] * v2 + H12[2]) * wi, v2in1 = (H12[3] * u2 + H12[4] * v2 + H12[5]) * wi;
-    const double chi1 = ((u1 - u2in1) * (u1 - u2in1) + (v1 - v2in1) * (v1 - v2in1)) * invSigmaSquare;
+    double chi1, chi2;                               // x2 in image 1 through H12, x1 in image 2 through H21 (:628-656)
+    epi::homography_score_chi(H21, H12, pts_img1[2 * i], pts_img1[2 * i + 1], pts_img2[2 * i], pts_img2[2 * i + 1], invSigmaSquare, &chi1, &chi2);
     if (chi1 > th) good = false;
     else score += th - chi1;
-    // x1 in image 2 through H21 (:642-656)
-    const double wj = 1.0 / (H21[6] * u1 + H21[7] * v1 + H21[8]);
-    const double u1in2 = (H21[0] * u1 + H21[1] * v1 + H21[2]) * wj, v1in2 = (H21[3] * u1 + H21[4] * v1 + H21[5]) * wj;
-    const double chi2 = ((u2 - u1in2) * (u2 - u1in2) + (v2 - v1in2) * (v2 - v1in2)) * invSigmaSquare;
     if (chi2 > th) good = false;
     else score += th - chi2;
     if (good) inliers[w++] = i;
@@ -107,17 +72,8 @@ int mvo_choose_e_or_h(double score_e, double score_h, const double *h_normals, i
 int mvo_choose_e_or_h_thr(double score_e, double score_h, const double *h_normals, int num_h, double threshold, int *best_sol,
                           double *ratio_out) {
   if (!best_sol || num_h < 0 || (num_h > 0 && !h_normals) || !(threshold > 0 && threshold < 1)) return MVO_ERR_INVALID_ARG;
-  // solution 0 is the essential one, 1..num_h the homography ones (motion_estimation.cpp:60-103)
-  const double ratio = score_h / (score_e + score_h);            // :137
   int best = 0;
-  if (ratio > threshold && num_h > 0) {                                // :140-152: the homography solution whose plane normal is most frontal
-    best = 1;
-    double largest = fabs(h_normals[2]);
-    for (int i = 2; i <= num_h; ++i) {
-      const double nz = fabs(h_normals[3 * (i - 1) + 2]);
-      if (nz > largest) { largest = nz; best = i; }
-    }
-  }
+  const double ratio = epi::eh_choose(score_e, score_h, h_normals, num_h, threshold, &best);
   *best_sol = best;
   if (ratio_out) *ratio_out = ratio;
   return MVO_OK;

@@ -101,8 +101,9 @@ struct mvo_ctx {
   PinBuf match_h;
   // batched matchFeatures (mvo_match_features_batch_dev): partial winners, merge tickets, packed keys of every pair
   DevBuf matchb_part, matchb_tickets, matchb_keys;
-  // batched essential-matrix motion (mvo_esti_motion_by_essential_batch_dev): points, hypotheses, counts and finish outputs of
-  // every pair; its own block, so that it never aliases the single-pair jobs' d_a / d_e that may run on the side stream
+  // batched two-view calls (mvo_esti_motion_by_essential_batch_dev, mvo_estimate_relative_poses_batch_dev): points, hypotheses,
+  // counts and finish outputs of every pair; its own block, so that it never aliases the single-pair jobs' d_a / d_e that may run
+  // on the side stream
   DevBuf epib_buf;
 
   // timing
@@ -332,6 +333,24 @@ int mvo_epi_homography_end(mvo_ctx *ctx, MvoEpiJob *job, const double *K, double
                            int32_t *inliers, int *n_inliers);
 int mvo_do_triangulation_multi(mvo_ctx *ctx, const float *pts_np1, const float *pts_np2, int n, int nsol, const double *const *R,
                                const double *const *t, const int32_t *const *inliers, const int *n_inliers, float *const *pts3d);
+// mvo_estimate_relative_poses_batch_dev (epipolar.cu) in three steps: the RANSAC halves (epipolar.cu), the combine step
+// (two_view_batch.cu: one launch, one CTA per pair), the triangulation of every solution (epipolar.cu).  MvoRelPosesCombine holds
+// what the first step leaves on the device for the others: the outputs of the essential half (ess, inl_e: pair p's list at
+// p * cap) and of the homography half (hom_d / hom_i: the finish outputs at p * hom_d_stride / p * hom_i_stride, inl_h), the
+// gathered pixel (p1, p2) and normalised-plane (np1, np2) points.  The combine step writes res, the inlier rows and rt: (R | t) of
+// every solution before basics::invRt, 12 doubles at (p * 5 + s) * 12, which the triangulation reads.
+struct MvoRelPosesCombine {
+  const int32_t *n_matches;
+  const mvo_two_view_result *ess;
+  const int32_t *inl_e, *hom_i, *inl_h;
+  const double *hom_d;
+  const float *p1, *p2, *np1, *np2;
+  int n_pairs, cap, hom_d_stride, hom_i_stride, motion_cam2_to_cam1;
+  double K[9], eh_ratio_threshold;
+  mvo_relative_poses_result *res;
+  int32_t *inliers;
+  double *rt;
+};
 cudaStream_t mvo_side_stream(mvo_ctx *ctx);      // a second non-blocking stream of the context, created on first use (ctx.cu)
 int mvo_epi_essential_ex(mvo_ctx *ctx, const float *pts1, const float *pts2, int n, const double *K, double threshold,
                          double *E, double *R, double *t, int32_t *inliers, int *n_inliers, int want_pose,

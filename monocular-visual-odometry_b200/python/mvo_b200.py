@@ -27,6 +27,13 @@ TWO_VIEW_RESULT_DTYPE = np.dtype(
     [("status", "<i4"), ("n_matches", "<i4"), ("n_inliers", "<i4"), ("votes", "<i4"), ("E", "<f8", (9,)), ("R", "<f8", (9,)),
      ("t", "<f8", (3,))])
 assert TWO_VIEW_RESULT_DTYPE.itemsize == 184
+# mvo_relative_poses_result (estimate_relative_poses_batch_dev): status, n_matches, then mvo_two_view_solutions as it is laid out
+# in memory (TwoViewSolutions below)
+RELATIVE_POSES_RESULT_DTYPE = np.dtype(
+    [("status", "<i4"), ("n_matches", "<i4"), ("num_solutions", "<i4"), ("best", "<i4"), ("n_inliers", "<i4", (5,)), ("pad_", "<i4"),
+     ("R", "<f8", (5, 9)), ("t", "<f8", (5, 3)), ("normal", "<f8", (5, 3)), ("E", "<f8", (9,)), ("H", "<f8", (9,)), ("score_e", "<f8"),
+     ("score_h", "<f8"), ("ratio", "<f8")])
+assert RELATIVE_POSES_RESULT_DTYPE.itemsize == 808
 
 MVO_OK = 0
 ERR_NAMES = {0: "MVO_OK", -1: "MVO_ERR_INVALID_ARG", -2: "MVO_ERR_NO_DEVICE", -3: "MVO_ERR_CUDA",
@@ -109,6 +116,7 @@ SIGNATURES = {
     "mvo_orb_extract_batch_dev": (_i, [_vp, _vp, _i, _i, _i, _i, _sz, _sz, _vp, _vp, _vp, _i]),
     "mvo_match_features_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _f, _vp, _vp]),
     "mvo_esti_motion_by_essential_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, C.c_double, _vp, _vp, _vp]),
+    "mvo_estimate_relative_poses_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "mvo_match_hamming_nn": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "mvo_match_hamming_knn2": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "mvo_match_radius_sad": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _f, _vp, _pi]),
@@ -321,6 +329,17 @@ class Context:
         self._chk(self.lib.mvo_esti_motion_by_essential_batch_dev(self.h, _ptr(d_kpts), _ptr(d_counts), batch, cap, _ptr(d_pairs), n_pairs,
                                                                   _ptr(d_matches), _ptr(d_n_matches), _ptr(K), float(threshold), _ptr(d_res),
                                                                   _ptr(d_inliers), _ptr(d_pts3d)))
+
+    def estimate_relative_poses_batch_dev(self, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K,
+                                          d_res, d_inliers, d_pts3d=None, motion_cam2_to_cam1=True):
+        """estimate_relative_poses(calc_homo=True) for n_pairs matched frame pairs of a batched extraction, all device pointers
+        except K (host 3x3): pair p's RELATIVE_POSES_RESULT_DTYPE record in d_res[p], solution s's inlier indices at
+        d_inliers + (p * 5 + s) * cap and its triangulated inliers at d_pts3d + (p * 5 + s) * cap * 3.  Thresholds, hypothesis
+        count and seed come from the context's parameters."""
+        K = _c(K, np.float64)
+        self._chk(self.lib.mvo_estimate_relative_poses_batch_dev(self.h, _ptr(d_kpts), _ptr(d_counts), batch, cap, _ptr(d_pairs), n_pairs,
+                                                                 _ptr(d_matches), _ptr(d_n_matches), _ptr(K), int(bool(motion_cam2_to_cam1)),
+                                                                 _ptr(d_res), _ptr(d_inliers), _ptr(d_pts3d)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):

@@ -6,9 +6,13 @@ threshold 1.0), and the essential-matrix motion plus the triangulation of every 
   batch     one mvo_esti_motion_by_essential_batch_dev call on the device-resident keypoints and match lists;
   per pair  download of the counts, keypoints and match lists, then per pair pts1 / pts2 on the host, mvo_esti_motion_by_essential
             and mvo_do_triangulation (two synchronisations per pair).
-Both are timed with CUDA events on the context stream after warm-up, alternating in the same run.  Reported: us per pair for
-both, launches per batch call, the card's name and power limit read in the same run.  Every pair's result of the batch call
-(status, E, R, t, inliers, triangulated points) is compared byte for byte with the per-pair path; a mismatch fails the run.
+and, with the homography branch and the E / H choice (what the reference's callers use), as
+  rp batch     one mvo_estimate_relative_poses_batch_dev call (motion_cam2_to_cam1 = 1, triangulation of every solution);
+  rp per pair  the same download, then mvo_estimate_relative_poses(calc_homo = 1) per pair.
+Each pair of paths is timed with CUDA events on the context stream after warm-up, alternating in the same run.  Reported: us per
+pair for every path, launches per batch call, the card's name and power limit read in the same run.  Every pair's result of a
+batch call (status, E, R, t, inliers, triangulated points; for the relative poses the whole mvo_two_view_solutions record and
+every solution's rows) is compared byte for byte with its per-pair path; a mismatch fails the run.
 Needs a GPU.  Usage: python tools/two_view_stream.py [--reps N] -> one JSON line."""
 import argparse
 import json
@@ -67,6 +71,29 @@ def per_pair(ctx, d_k, d_c, d_m, d_n, pairs):
     return out
 
 
+def per_pair_rp(ctx, d_k, d_c, d_m, d_n, pairs):
+    """Today's host path for the relative poses: the same download, then mvo_estimate_relative_poses(calc_homo = 1) per pair.
+    Returns, per pair, (status, the mvo_two_view_solutions bytes, inlier rows 5 x n, triangulated rows 5 x n x 3)."""
+    import ctypes as C
+    kp = d_k.cpu().numpy().view(mvo_b200.KEYPOINT_DTYPE).reshape(B, CAP)
+    matches = d_m.cpu().numpy().view(mvo_b200.DMATCH_DTYPE).reshape(len(pairs), CAP)
+    n_m = d_n.cpu().numpy()
+    Kc = np.ascontiguousarray(K, np.float64)
+    out = []
+    for p, (q, t) in enumerate(pairs):
+        m = matches[p, :n_m[p]]
+        n = len(m)
+        p1 = np.ascontiguousarray(np.stack([kp[q]["x"][m["query_idx"]], kp[q]["y"][m["query_idx"]]], 1), np.float32)
+        p2 = np.ascontiguousarray(np.stack([kp[t]["x"][m["train_idx"]], kp[t]["y"][m["train_idx"]]], 1), np.float32)
+        sol = mvo_b200.TwoViewSolutions()
+        inl = np.zeros((5, max(n, 1)), np.int32)
+        pts = np.zeros((5, max(n, 1), 3), np.float32)
+        rc = ctx.lib.mvo_estimate_relative_poses(ctx.h, p1.ctypes.data, p2.ctypes.data, n, Kc.ctypes.data, 1, 1, C.byref(sol),
+                                                 inl.ctypes.data, pts.ctypes.data)
+        out.append((rc, bytes(sol) if rc == 0 else None, inl, pts))
+    return out
+
+
 def main():
     import torch
     ap = argparse.ArgumentParser()
@@ -90,6 +117,9 @@ def main():
     d_res = torch.zeros(n * mvo_b200.TWO_VIEW_RESULT_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
     d_inl = torch.zeros(n * CAP, dtype=torch.int32, device="cuda")
     d_pts = torch.zeros(n * CAP * 3, dtype=torch.float32, device="cuda")
+    d_res2 = torch.zeros(n * mvo_b200.RELATIVE_POSES_RESULT_DTYPE.itemsize, dtype=torch.uint8, device="cuda")
+    d_inl2 = torch.zeros(n * 5 * CAP, dtype=torch.int32, device="cuda")
+    d_pts2 = torch.zeros(n * 5 * CAP * 3, dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()
     ctx.orb_extract_batch_dev(d_img.data_ptr(), B, H, W, 3, W * 3, H * W * 3, d_k.data_ptr(), d_d.data_ptr(), d_c.data_ptr(), CAP)
     ctx.match_features_batch_dev(d_k.data_ptr(), d_d.data_ptr(), d_c.data_ptr(), B, CAP, d_p.data_ptr(), n, 1, 0.0, d_m.data_ptr(),
@@ -99,6 +129,10 @@ def main():
     def batch():
         ctx.esti_motion_by_essential_batch_dev(d_k.data_ptr(), d_c.data_ptr(), B, CAP, d_p.data_ptr(), n, d_m.data_ptr(), d_n.data_ptr(), K,
                                                THRESHOLD, d_res.data_ptr(), d_inl.data_ptr(), d_pts.data_ptr())
+
+    def batch_rp():
+        ctx.estimate_relative_poses_batch_dev(d_k.data_ptr(), d_c.data_ptr(), B, CAP, d_p.data_ptr(), n, d_m.data_ptr(), d_n.data_ptr(), K,
+                                              d_res2.data_ptr(), d_inl2.data_ptr(), d_pts2.data_ptr(), motion_cam2_to_cam1=True)
 
     def ev_time(fn):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -112,16 +146,25 @@ def main():
     for _ in range(2):                                             # warm-up: module loads, scratch growth
         batch()
         ref = per_pair(ctx, d_k, d_c, d_m, d_n, pairs)
+        batch_rp()
+        ref_rp = per_pair_rp(ctx, d_k, d_c, d_m, d_n, pairs)
     ctx.synchronize()
     l0 = ctx.lib.mvo_kernel_launches(ctx.h)
     batch()
     launches = int(ctx.lib.mvo_kernel_launches(ctx.h) - l0)
-    t_batch, t_host = [], []
+    l0 = ctx.lib.mvo_kernel_launches(ctx.h)
+    batch_rp()
+    launches_rp = int(ctx.lib.mvo_kernel_launches(ctx.h) - l0)
+    t_batch, t_host, t_batch_rp, t_host_rp = [], [], [], []
     for _ in range(args.reps):                                     # alternating
         us, _ = ev_time(batch)
         t_batch.append(us)
         us, ref = ev_time(lambda: per_pair(ctx, d_k, d_c, d_m, d_n, pairs))
         t_host.append(us)
+        us, _ = ev_time(batch_rp)
+        t_batch_rp.append(us)
+        us, ref_rp = ev_time(lambda: per_pair_rp(ctx, d_k, d_c, d_m, d_n, pairs))
+        t_host_rp.append(us)
 
     res = d_res.cpu().numpy().view(mvo_b200.TWO_VIEW_RESULT_DTYPE)
     inl = d_inl.cpu().numpy().reshape(n, CAP)
@@ -138,6 +181,21 @@ def main():
                   and inl[p, :ni].tobytes() == il.tobytes() and pts[p, :ni].tobytes() == pt.tobytes())
         if not ok:
             bad.append(p)
+    res2 = d_res2.cpu().numpy().view(mvo_b200.RELATIVE_POSES_RESULT_DTYPE)
+    inl2 = d_inl2.cpu().numpy().reshape(n, 5, CAP)
+    pts2 = d_pts2.cpu().numpy().reshape(n, 5, CAP, 3)
+    bad_rp = []
+    for p, (rc, sol, il, pt) in enumerate(ref_rp):
+        r = res2[p]
+        ok = r["status"] == rc and r["n_matches"] == d_n[p].item()
+        if ok and rc == 0:
+            ok = r.tobytes()[8:] == sol
+            for s_ in range(int(r["num_solutions"])):
+                ni = int(r["n_inliers"][s_])
+                ok = ok and inl2[p, s_, :ni].tobytes() == il[s_, :ni].tobytes() and pts2[p, s_, :ni].tobytes() == pt[s_, :ni].tobytes()
+        if not ok:
+            bad_rp.append(p)
+    okp = res2["status"] == 0
     med = lambda v: float(np.median(v))  # noqa: E731
     line = {"tool": "two_view_stream", "frames": B, "pairs": n, "pair_kinds": "(i, i+1) and (i, i+8)", "cap": CAP, "max_keypoints": 2000,
             "match_method": 1, "threshold_px": THRESHOLD, "epi_hypotheses": int(ctx.params.epi_hypotheses), "card": card(),
@@ -146,11 +204,18 @@ def main():
             "batch_us_per_call": med(t_batch), "batch_us_per_pair": med(t_batch) / n, "batch_launches_per_call": launches,
             "per_pair_host_us_per_call": med(t_host), "per_pair_host_us_per_pair": med(t_host) / n,
             "speedup": med(t_host) / med(t_batch), "pairs_differing_from_per_pair_path": len(bad),
+            "rp_homography_threshold_px": float(ctx.params.homography_threshold), "rp_eh_ratio_threshold": float(ctx.params.eh_ratio_threshold),
+            "rp_pairs_ok": int(okp.sum()), "rp_pairs_h_chosen": int((res2["best"][okp] > 0).sum()),
+            "rp_homography_solutions_per_ok_pair": float((res2["num_solutions"][okp] - 1).mean()),
+            "rp_batch_us_per_call": med(t_batch_rp), "rp_batch_us_per_pair": med(t_batch_rp) / n, "rp_batch_launches_per_call": launches_rp,
+            "rp_per_pair_host_us_per_call": med(t_host_rp), "rp_per_pair_host_us_per_pair": med(t_host_rp) / n,
+            "rp_speedup": med(t_host_rp) / med(t_batch_rp), "rp_pairs_differing_from_per_pair_path": len(bad_rp),
             "timing": f"CUDA events on the context stream, median of {args.reps} alternating repetitions after 2 warm-up rounds"}
     print(json.dumps(line), flush=True)
     ctx.close()
-    if bad:
-        raise SystemExit(f"two_view_stream: batch results differ from the per-pair path for pairs {bad[:10]}")
+    if bad or bad_rp:
+        raise SystemExit(f"two_view_stream: batch results differ from the per-pair path for pairs {bad[:10]} (essential), "
+                         f"{bad_rp[:10]} (relative poses)")
 
 
 if __name__ == "__main__":
