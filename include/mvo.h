@@ -517,6 +517,55 @@ typedef struct mvo_vo_params {
   double assumed_mean_depth_init;      /* assumed_mean_pts_depth_during_vo_init = 0.8 */
 } mvo_vo_params;
 
+/* The initialisation check of the state machine (estimateMotionAnd3DPoints_ + isVoGoodToInit_, src/vo/vo.cpp:53-172) for the
+ * matched frame pairs of a batch, entirely on the device: the step after mvo_estimate_relative_poses_batch_dev.  Pair p = (query
+ * frame, train frame) is (reference keyframe, candidate frame); its record says what the state machine decides when that candidate
+ * is the frame being added and T_w_c_ref is the reference keyframe's pose:
+ *   the chosen solution's inlier matches (img_idx = -1), its triangulated points moved into the candidate's camera (transCoord),
+ *   T_w_c = T_w_c_ref * [R|t]^-1, retainGoodTriangulationResult_ (angles, their median, the drop by angle), the depth
+ *   normalisation when at least 20 points survive, and the three criteria of isVoGoodToInit_.
+ * Inputs: d_kpts / d_counts / batch / cap / d_pairs / n_pairs / d_matches / d_n_matches exactly as given to
+ * mvo_estimate_relative_poses_batch_dev, and what it wrote (d_rp, d_rp_inliers, d_rp_pts3d, same row layouts).  Precondition:
+ * that call was made with motion_cam2_to_cam1 = 1 and a non-NULL d_pts3d (the state machine's call).  T_w_c_ref: host 4x4
+ * row-major; vp: host, the fields min_triang_angle, max_ratio_angle_to_median, min_inlier_matches, min_pixel_dist,
+ * min_median_triangulation_angle and assumed_mean_depth_init (init_calc_homography is not read: the inputs are those of the
+ * homography branch, the reference's is_calc_homo = true).
+ * Outputs of pair p: d_out[p]; inliers_matches_for_3d_ at d_kept + p * cap, inliers_pts3d_ (candidate camera, after the
+ * normalisation) at d_kept_pts3d + p * cap * 3 and triangulation_angles_of_inliers_ at d_kept_angles + p * cap, n_kept of each, in
+ * the reference's order; nothing past n_kept is written.
+ * Per pair: a relative-poses status MVO_ERR_DEGENERATE gives usable = 0, good = 0, best_sol = -1, T_w_c = T_w_c_ref and status
+ * MVO_OK (as the state machine treats it); any other non-MVO_OK status is propagated.  MVO_ERR_INVALID_ARG for that pair alone,
+ * checked before anything is read through the value checked: a frame index outside [0, batch), d_n_matches[p] outside [0, cap],
+ * best outside [0, num_solutions) or num_solutions outside [1, 5], n_inliers[best] outside [0, d_n_matches[p]], an inlier index
+ * outside [0, d_n_matches[p]), a keypoint index of an inlier match outside its frame.  A failed pair writes its status only.
+ * Numerics: the host's order of operations, without contraction; every sum over points is sequential in list order.  Each
+ * angle uses the device's acos (2 ulp), the one step that is not the host's (glibc) bit for bit: the angles and median_angle
+ * are within a few ulp of the state machine's, and everything else is byte-identical unless an angle lies that close to a
+ * threshold.  A NaN angle, median_angle or mean_pixel_dist (0 / 0 when n_kept = 0) has x86-64's default NaN bits.
+ * MVO_ERR_INVALID_ARG: a null pointer, a T_w_c_ref or vp value that is not finite, batch or cap < 1, n_pairs < 0.
+ * MVO_ERR_UNSUPPORTED: cap > 6400 or n_pairs > 65535 (the limits of mvo_estimate_relative_poses_batch_dev), or a library built
+ * without the kernel's translation unit.  Asynchronous on the context stream: one kernel launch whatever n_pairs is, no host
+ * synchronisation. */
+typedef struct mvo_init_candidate_result {
+  int32_t status;      /* MVO_OK, or the pair's mvo_status */
+  int32_t usable;      /* estimateMotionAnd3DPoints_ got past the two-view step (0: degenerate pair) */
+  int32_t good;        /* isVoGoodToInit_ */
+  int32_t best_sol;    /* the E/H choice of the relative-poses record; -1 when not usable */
+  int32_t n_inliers;   /* inliers of the chosen solution (inliers_matches_with_ref_) */
+  int32_t n_kept;      /* after retainGoodTriangulationResult_ (inliers_matches_for_3d_) */
+  int32_t normalized;  /* n_kept >= 20: depth normalised (vo.cpp:97-108) */
+  int32_t pad;
+  double scale;                          /* assumed_mean_depth_init / mean depth; 0 when not normalised */
+  double mean_pixel_dist, median_angle;  /* what isVoGoodToInit_ compares; median_angle = 0 when n_kept = 0 */
+  double t_curr_to_prev[3];              /* the chosen t after the depth scaling */
+  double T_w_c[16];                      /* the candidate's pose as estimateMotionAnd3DPoints_ leaves it (T_w_c_ref if not usable) */
+} mvo_init_candidate_result;
+int mvo_vo_init_candidates_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                     const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches, const int32_t *d_n_matches,
+                                     const mvo_relative_poses_result *d_rp, const int32_t *d_rp_inliers, const float *d_rp_pts3d,
+                                     const double *T_w_c_ref, const mvo_vo_params *vp, mvo_init_candidate_result *d_out,
+                                     mvo_dmatch *d_kept, float *d_kept_pts3d, double *d_kept_angles);
+
 typedef struct mvo_vo_frame_info {
   int32_t frame_id, state_in, state_out;   /* states: 0 BLANK, 1 DOING_INITIALIZATION, 2 DOING_TRACKING (vo.h:52-58) */
   int32_t keyframe;                        /* this frame became a keyframe */

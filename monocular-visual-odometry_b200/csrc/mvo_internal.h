@@ -133,16 +133,31 @@ int mvo_reserve(mvo_ctx *ctx, DevBuf &b, size_t bytes);
 int mvo_reserve_pinned(mvo_ctx *ctx, PinBuf &b, size_t bytes);
 
 // Host arithmetic on rigid transforms (4x4 row-major doubles) shared by the tracker and the VO state machine, in the reference's
-// operation order: tracker.cpp and vo_pipeline.cpp get the same bits.
+// operation order: tracker.cpp and vo_pipeline.cpp get the same bits.  inv_rigid and rt_to_T also serve vo_init_batch.cu, which
+// is compiled without contraction and so gets the host's bits as well.
+#if defined(__CUDACC__)
+#define MVO_HD __host__ __device__
+#else
+#define MVO_HD
+#endif
+// What 0 / 0 (and every NaN made from finite inputs) is on x86-64: the default NaN, sign bit set.  The device makes NaNs with other
+// bits; the kernels that restate host arithmetic (two_view_batch.cu, vo_init_batch.cu) write the host's into their double outputs.
+static inline MVO_HD double as_host_nan(double v) {
+  if (v == v) return v;
+  const unsigned long long bits = 0xFFF8000000000000ull;
+  double d;
+  memcpy(&d, &bits, sizeof d);
+  return d;
+}
 static inline void set_identity(double *T) { memset(T, 0, 16 * sizeof(double)); T[0] = T[5] = T[10] = T[15] = 1; }
-static inline void inv_rigid(const double *T, double *Ti) {        // [R t; 0 1]^-1 = [R^T, -R^T t]; Ti may be T
+static inline MVO_HD void inv_rigid(const double *T, double *Ti) {        // [R t; 0 1]^-1 = [R^T, -R^T t]; Ti may be T
   double r[16];
   for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) r[i * 4 + j] = T[j * 4 + i];
   for (int i = 0; i < 3; ++i) r[i * 4 + 3] = -(r[i * 4] * T[3] + r[i * 4 + 1] * T[7] + r[i * 4 + 2] * T[11]);
   r[12] = r[13] = r[14] = 0; r[15] = 1;
   memcpy(Ti, r, sizeof r);
 }
-static inline void rt_to_T(const double *R, const double *t, double *T) {      // basics::convertRt2T
+static inline MVO_HD void rt_to_T(const double *R, const double *t, double *T) {      // basics::convertRt2T
   for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) T[i * 4 + j] = R[i * 3 + j]; T[i * 4 + 3] = t[i]; }
   T[12] = T[13] = T[14] = 0; T[15] = 1;
 }
@@ -351,6 +366,23 @@ struct MvoRelPosesCombine {
   int32_t *inliers;
   double *rt;
 };
+// mvo_vo_init_candidates_batch_dev (vo_pipeline.cpp checks the arguments, vo_init_batch.cu launches one CTA per pair): the inputs
+// as the call received them, T_w_c_ref and the thresholds by value
+struct MvoInitCandidates {
+  const mvo_keypoint *kpts;
+  const int32_t *counts, *pairs, *n_matches, *rp_inliers;
+  const mvo_dmatch *matches;
+  const mvo_relative_poses_result *rp;
+  const float *rp_pts3d;
+  int batch, cap, n_pairs, min_inlier_matches;
+  double T_ref[16];
+  double min_triang_angle, max_ratio_angle_to_median, min_pixel_dist, min_median_triangulation_angle, assumed_mean_depth_init;
+  mvo_init_candidate_result *out;
+  mvo_dmatch *kept;
+  float *kept_pts3d;
+  double *kept_angles;
+};
+int mvo_vo_init_candidates_launch(mvo_ctx *ctx, const MvoInitCandidates &a);
 cudaStream_t mvo_side_stream(mvo_ctx *ctx);      // a second non-blocking stream of the context, created on first use (ctx.cu)
 int mvo_epi_essential_ex(mvo_ctx *ctx, const float *pts1, const float *pts2, int n, const double *K, double threshold,
                          double *E, double *R, double *t, int32_t *inliers, int *n_inliers, int want_pose,

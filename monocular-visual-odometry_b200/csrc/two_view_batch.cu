@@ -18,16 +18,6 @@ namespace {
 
 constexpr int RPC_T = 256;
 
-// what 0 / 0 (and every NaN made from finite inputs) is on x86-64: the default NaN, sign bit set.  The device makes NaNs with
-// other bits; score_e, score_h and the ratio get the host's.
-__device__ __forceinline__ double as_host_nan(double v) {
-  if (v == v) return v;
-  const unsigned long long bits = 0xFFF8000000000000ull;
-  double d;
-  memcpy(&d, &bits, sizeof d);
-  return d;
-}
-
 struct RpcSmem {
   mvo_two_view_solutions sol;            // the pair's record, zeroed first as the host memsets its struct
   double Rh[36], th[12], nh[12], F[9], H12[9];

@@ -4,13 +4,15 @@
 //   the depth normalisation of estimateMotionAnd3DPoints_   src/vo/vo.cpp:96-110
 //   isVoGoodToInit_                  src/vo/vo.cpp:113-172
 //   checkLargeMoveForAddKeyFrame_    src/vo/vo.cpp:247-265
-// No GPU work and no context: double arithmetic in the reference's order of operations.
+// No GPU work and no context: double arithmetic in the reference's order of operations.  The per-point terms live in
+// vo_init_math.cuh, shared with mvo_vo_init_candidates_batch_dev (vo_init_batch.cu).
 #include <algorithm>
 #include <math.h>
 #include <numeric>
 #include <stdint.h>
 #include <vector>
 #include "mvo.h"
+#include "vo_init_math.cuh"
 
 extern "C" {
 
@@ -20,24 +22,7 @@ int mvo_retain_good_triangulation(const float *pts3d_in_curr, int n, const doubl
   *n_keep = 0;
   if (n == 0) return MVO_OK;                                    // vo.cpp:203-205
   std::vector<double> all((size_t)n);
-  for (int i = 0; i < n; ++i) {
-    // basics::preTranslatePoint3f(p, T_w_c): double accumulation, narrowed to Point3f; then back to a double 3x1 (:208-209)
-    const double p0 = pts3d_in_curr[3 * i], p1 = pts3d_in_curr[3 * i + 1], p2 = pts3d_in_curr[3 * i + 2];
-    double pw[3];
-    for (int r = 0; r < 3; ++r) {
-      double acc = 0;
-      acc += T_w_c_curr[r * 4] * p0; acc += T_w_c_curr[r * 4 + 1] * p1; acc += T_w_c_curr[r * 4 + 2] * p2; acc += T_w_c_curr[r * 4 + 3] * 1.0;
-      pw[r] = (double)(float)acc;
-    }
-    double v1[3], v2[3], dot = 0, n1 = 0, n2 = 0;
-    for (int r = 0; r < 3; ++r) {
-      v1[r] = T_w_c_curr[r * 4 + 3] - pw[r];                     // getPosFromT(curr) - p (:210)
-      v2[r] = T_w_c_ref[r * 4 + 3] - pw[r];                      // getPosFromT(ref) - p  (:211)
-      dot += v1[r] * v2[r]; n1 += v1[r] * v1[r]; n2 += v2[r] * v2[r];
-    }
-    const double angle = acos(dot / (sqrt(n1) * sqrt(n2)));      // calcAngleBetweenTwoVectors (opencv_funcs.cpp:176-190)
-    all[(size_t)i] = angle / 3.1415926 * 180.0;                  // :213 (the reference's truncated pi)
-  }
+  for (int i = 0; i < n; ++i) all[(size_t)i] = voi::triangulation_angle(pts3d_in_curr + 3 * i, T_w_c_curr, T_w_c_ref);    // :206-214
   std::vector<double> sorted = all;
   std::nth_element(sorted.begin(), sorted.begin() + n / 2, sorted.end());      // the reference sorts and reads element n / 2 (:216-220): same value
   const double median = sorted[(size_t)(n / 2)];
@@ -71,10 +56,7 @@ int mvo_is_vo_good_to_init(const float *kpts_ref_xy, const float *kpts_curr_xy, 
     return MVO_ERR_INVALID_ARG;
   const bool criteria_0 = n_matches >= min_inlier_matches;       // vo.cpp:127-133
   double mean_dist = 0;                                          // computeMeanDistBetweenKeypoints (feature_match.cpp:262-279)
-  for (int i = 0; i < n_matches; ++i) {
-    const double dx = kpts_ref_xy[2 * i] - kpts_curr_xy[2 * i], dy = kpts_ref_xy[2 * i + 1] - kpts_curr_xy[2 * i + 1];
-    mean_dist += sqrt(dx * dx + dy * dy);
-  }
+  for (int i = 0; i < n_matches; ++i) mean_dist += voi::pixel_dist(kpts_ref_xy[2 * i], kpts_ref_xy[2 * i + 1], kpts_curr_xy[2 * i], kpts_curr_xy[2 * i + 1]);
   mean_dist /= n_matches;                                        // 0/0 = NaN for no matches, like the reference: the comparison below is false
   const bool criteria_1 = mean_dist > min_pixel_dist;            // :136-143
   bool criteria_2 = false;                                       // :146-168

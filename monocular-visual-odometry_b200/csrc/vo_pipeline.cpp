@@ -34,11 +34,13 @@
 #include <string.h>
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <deque>
 #include <memory>
 #include <unordered_map>
 #include <vector>
 #include "mvo_internal.h"
+#include "vo_init_math.cuh"
 
 namespace {
 
@@ -91,19 +93,8 @@ struct VoMapPoint {                                              // vo::MapPoint
   int visible_times = 1, matched_times = 1;
 };
 
-void mul44(const double *A, const double *B, double *C) {
-  double r[16];
-  for (int i = 0; i < 4; ++i) for (int j = 0; j < 4; ++j) {
-    double a = 0;
-    for (int k = 0; k < 4; ++k) a += A[i * 4 + k] * B[k * 4 + j];
-    r[i * 4 + j] = a;
-  }
-  memcpy(C, r, sizeof r);
-}
-// basics::transCoord (opencv_funcs.cpp:121-125): R * p + t in double, narrowed to Point3f
-void trans_coord(const float *p, const double *R, const double *t, float *out) {
-  for (int r = 0; r < 3; ++r) out[r] = (float)(R[r * 3] * (double)p[0] + R[r * 3 + 1] * (double)p[1] + R[r * 3 + 2] * (double)p[2] + t[r]);
-}
+using voi::mul44;
+using voi::trans_coord;
 void rodrigues_to_R(const double *w, double *R) {                // cv::Rodrigues(rvec -> R)
   const double th = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
   if (th < 1e-300) { R[0] = R[4] = R[8] = 1; R[1] = R[2] = R[3] = R[5] = R[6] = R[7] = 0; return; }
@@ -995,3 +986,43 @@ int mvo_vo_frame_pose(const mvo_vo *v, int k, double *T_w_c) {
 }
 
 }  // extern "C"
+
+// The kernel of mvo_vo_init_candidates_batch_dev lives in vo_init_batch.cu, a translation unit of its own that is compiled without
+// contraction (Makefile).  libmvo.so always links it; a library assembled from a subset of the units without it reports
+// MVO_ERR_UNSUPPORTED for the call.
+int mvo_vo_init_candidates_launch(mvo_ctx *ctx, const MvoInitCandidates &a) __attribute__((weak));
+
+// mvo_vo_init_candidates_batch_dev (mvo.h): the call-level checks here, everything per pair in one launch (vo_init_batch.cu)
+extern "C" int mvo_vo_init_candidates_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                                const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
+                                                const int32_t *d_n_matches, const mvo_relative_poses_result *d_rp,
+                                                const int32_t *d_rp_inliers, const float *d_rp_pts3d, const double *T_w_c_ref,
+                                                const mvo_vo_params *vp, mvo_init_candidate_result *d_out, mvo_dmatch *d_kept,
+                                                float *d_kept_pts3d, double *d_kept_angles) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (!d_kpts || !d_counts || !d_pairs || !d_matches || !d_n_matches || !d_rp || !d_rp_inliers || !d_rp_pts3d || !T_w_c_ref || !vp ||
+      !d_out || !d_kept || !d_kept_pts3d || !d_kept_angles)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo init candidates batch: null pointer");
+  if (!mvo_vo_init_candidates_launch)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "vo init candidates batch: the library was built without vo_init_batch.cu");
+  if (n_pairs < 0 || batch < 1 || cap < 1)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo init candidates batch: n_pairs=%d batch=%d cap=%d", n_pairs, batch, cap);
+  for (int q = 0; q < 16; ++q)
+    if (!std::isfinite(T_w_c_ref[q])) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo init candidates batch: T_w_c_ref is not finite");
+  const double thr[5] = {vp->min_triang_angle, vp->max_ratio_angle_to_median, vp->min_pixel_dist, vp->min_median_triangulation_angle,
+                         vp->assumed_mean_depth_init};
+  for (double x : thr)
+    if (!std::isfinite(x)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo init candidates batch: a threshold of vp is not finite");
+  if (cap > 6400) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "vo init candidates batch: cap %d above 6400 correspondences", cap);
+  if (n_pairs > 65535) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "vo init candidates batch: %d pairs, at most 65535 per call", n_pairs);
+  if (n_pairs == 0) return MVO_OK;
+  MvoInitCandidates a;
+  a.kpts = d_kpts; a.counts = d_counts; a.pairs = d_pairs; a.n_matches = d_n_matches; a.rp_inliers = d_rp_inliers; a.matches = d_matches;
+  a.rp = d_rp; a.rp_pts3d = d_rp_pts3d;
+  a.batch = batch; a.cap = cap; a.n_pairs = n_pairs; a.min_inlier_matches = vp->min_inlier_matches;
+  memcpy(a.T_ref, T_w_c_ref, sizeof a.T_ref);
+  a.min_triang_angle = thr[0]; a.max_ratio_angle_to_median = thr[1]; a.min_pixel_dist = thr[2]; a.min_median_triangulation_angle = thr[3];
+  a.assumed_mean_depth_init = thr[4];
+  a.out = d_out; a.kept = d_kept; a.kept_pts3d = d_kept_pts3d; a.kept_angles = d_kept_angles;
+  return mvo_vo_init_candidates_launch(ctx, a);
+}

@@ -34,6 +34,12 @@ RELATIVE_POSES_RESULT_DTYPE = np.dtype(
      ("R", "<f8", (5, 9)), ("t", "<f8", (5, 3)), ("normal", "<f8", (5, 3)), ("E", "<f8", (9,)), ("H", "<f8", (9,)), ("score_e", "<f8"),
      ("score_h", "<f8"), ("ratio", "<f8")])
 assert RELATIVE_POSES_RESULT_DTYPE.itemsize == 808
+# mvo_init_candidate_result (vo_init_candidates_batch_dev): one record per frame pair
+INIT_CANDIDATE_RESULT_DTYPE = np.dtype(
+    [("status", "<i4"), ("usable", "<i4"), ("good", "<i4"), ("best_sol", "<i4"), ("n_inliers", "<i4"), ("n_kept", "<i4"),
+     ("normalized", "<i4"), ("pad", "<i4"), ("scale", "<f8"), ("mean_pixel_dist", "<f8"), ("median_angle", "<f8"),
+     ("t_curr_to_prev", "<f8", (3,)), ("T_w_c", "<f8", (16,))])
+assert INIT_CANDIDATE_RESULT_DTYPE.itemsize == 208
 
 MVO_OK = 0
 ERR_NAMES = {0: "MVO_OK", -1: "MVO_ERR_INVALID_ARG", -2: "MVO_ERR_NO_DEVICE", -3: "MVO_ERR_CUDA",
@@ -174,6 +180,8 @@ SIGNATURES = {
     "mvo_vo_get_map": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _pi]),
     "mvo_vo_frame_pose": (_i, [_vp, _i, _vp]),
     "mvo_vo_frame_data": (_i, [_vp, _i, _i, _vp, _i, _pi]),
+    "mvo_vo_init_candidates_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(VoParams), _vp, _vp, _vp,
+                                              _vp]),
     "mvo_vo_has_keyframe": (_i, [_vp, _i]),
     "mvo_write_pose_file": (_i, [C.c_char_p, _vp, _i]),
     "mvo_read_pose_file": (_i, [C.c_char_p, _vp, _i, _pi]),
@@ -340,6 +348,19 @@ class Context:
         self._chk(self.lib.mvo_estimate_relative_poses_batch_dev(self.h, _ptr(d_kpts), _ptr(d_counts), batch, cap, _ptr(d_pairs), n_pairs,
                                                                  _ptr(d_matches), _ptr(d_n_matches), _ptr(K), int(bool(motion_cam2_to_cam1)),
                                                                  _ptr(d_res), _ptr(d_inliers), _ptr(d_pts3d)))
+
+    def vo_init_candidates_batch_dev(self, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, d_rp, d_rp_inliers,
+                                     d_rp_pts3d, T_w_c_ref, vo_params, d_out, d_kept, d_kept_pts3d, d_kept_angles):
+        """The initialisation check of the state machine (estimateMotionAnd3DPoints_ + isVoGoodToInit_) for every pair of an
+        estimate_relative_poses_batch_dev call (motion_cam2_to_cam1 = True, with d_pts3d), all device pointers except T_w_c_ref
+        (host 4x4) and vo_params (VoParams): pair p's INIT_CANDIDATE_RESULT_DTYPE record in d_out[p], its kept matches at
+        d_kept + p * cap, kept points at d_kept_pts3d + p * cap * 3 and kept angles at d_kept_angles + p * cap."""
+        T = _c(T_w_c_ref, np.float64)
+        assert T.size == 16
+        self._chk(self.lib.mvo_vo_init_candidates_batch_dev(self.h, _ptr(d_kpts), _ptr(d_counts), batch, cap, _ptr(d_pairs), n_pairs,
+                                                            _ptr(d_matches), _ptr(d_n_matches), _ptr(d_rp), _ptr(d_rp_inliers),
+                                                            _ptr(d_rp_pts3d), _ptr(T), C.byref(vo_params), _ptr(d_out), _ptr(d_kept),
+                                                            _ptr(d_kept_pts3d), _ptr(d_kept_angles)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):
