@@ -9,13 +9,15 @@
 // in both cameras, OpenCV's tie order).  What differs by design, as for PnP: all H hypotheses
 // (mvo_params::epi_hypotheses, default 4096 — not the adaptive <= ~1000 of prob 0.999) are generated and scored in one
 // batch; the minimal solver is the linear eight-point method projected onto the essential manifold instead of
-// Nister's five-point solver; and the best minimal model is locally optimised on its consensus set (k_epi_finish).
-//   k_epi_hypotheses  one thread per hypothesis: counter-based sampling, epi::essential_from_8
-//   k_epi_score       one warp per hypothesis, points staged once per CTA in shared memory, count(Sampson <= thr^2)
-//   k_epi_finish      one CTA: arg-max (ties -> lowest hypothesis), ordered inlier list, recoverPose vote
-//   k_triangulate     one thread per point: epi::triangulate_dlt
-// mvo_esti_motion_by_essential_batch_dev runs the same kernel bodies over a batch of matched frame pairs (a pair dimension on
-// every kernel, one finish cluster per pair, recoverPose's pick on the device: epipolar_kernels.cuh, "batch of frame pairs").
+// Nister's five-point solver; and the best minimal model is locally optimised on its consensus set (k_epi_finish_batch).
+//   k_epi_hypotheses_batch  one thread per hypothesis: counter-based sampling, epi::essential_from_8
+//   k_epi_score_batch       one warp per hypothesis, points staged once per CTA in shared memory, count(Sampson <= thr^2)
+//   k_epi_finish_batch      one 8-CTA cluster: arg-max (ties -> lowest hypothesis), local optimisation, ordered inlier list
+//   k_epi_vote_batch        recoverPose's cheirality vote, one thread per (inlier, candidate)
+//   k_triangulate           one thread per point: epi::triangulate_dlt
+// Every RANSAC kernel, essential and homography (k_homo_*_batch), has a pair dimension (one pair per blockIdx.y, one finish
+// cluster per pair).  The batch calls run them over the matched frame pairs of a batch, with recoverPose's pick on the device
+// (k_epi_pick); the single-pair calls run them as a batch of one (cap = n, pn[0] = n uploaded with the points) and pick on the host.
 // The numerics live in epipolar_math.cuh and are unit-tested on the host (tests/test_epipolar_math.py).
 #include <cooperative_groups.h>
 #include <stdlib.h>
@@ -149,46 +151,133 @@ int epi_batch_check(mvo_ctx *ctx, const char *what, int batch, int cap, int n_pa
   return MVO_OK;
 }
 
-// Scratch of the essential half: gathered points (np1 / np2 optional), pn, hypothesis rows (Es 72 B + valid 4 B + cnt 4 B per
-// hypothesis), finish outputs
-struct EpiBatchScratch {
-  float *p1, *p2, *np1, *np2;
-  int32_t *pn, *valid, *cnt, *oi;
-  double *Es, *od;
+// One RANSAC's device rows for n_pairs pairs (epipolar_kernels.cuh, "batch of frame pairs"): points and pn, hypothesis rows (72 B
+// model, valid, count), finish outputs and inlier lists.  A single-pair call lays them out for one pair with cap = n.
+struct RansacRows {
+  float *p1, *p2;
+  int32_t *pn;
+  double *models, *od;
+  int32_t *valid, *cnt, *oi, *inl;
 };
 
-// gather, hypotheses, scoring, finish, vote, pick: six launches; pair p's inliers at inl + p * cap, its record in res[p]
-int epi_essential_batch_enqueue(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap, const int32_t *d_pairs,
-                                int n_pairs, const mvo_dmatch *d_matches, const int32_t *d_n_matches, const double *K, double threshold,
-                                const EpiBatchScratch &b, mvo_two_view_result *res, int32_t *inl) {
-  EpiCam cam;
-  cam.f = (K[0] + K[4]) / 2; cam.cx = K[2]; cam.cy = K[5];
-  const int H = ctx->prm.epi_hypotheses;
-  const size_t smem = (size_t)cap * 4 * sizeof(double);
-  const double thr2 = (threshold / cam.f) * (threshold / cam.f);          // as mvo_epi_essential_begin
-  { KTimer kt(ctx, KC_EPI);
-  k_epi_gather<<<n_pairs, 256, 0, ctx->stream>>>(d_kpts, d_counts, batch, cap, (const int2 *)d_pairs, d_matches, d_n_matches, K[0], K[4], K[2], K[5],
-                                                 b.p1, b.p2, b.np1, b.np2, b.pn); }
-  MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI);
-  k_epi_hypotheses_batch<<<dim3((H + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(b.p1, b.p2, b.pn, cap, cam, ctx->prm.pnp_seed, H, b.Es, b.valid); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_epi_score_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  // about as many CTAs in all as the single call uses for its one pair, at least one per pair
+// The launch geometry of both RANSACs for n_pairs pairs of at most cap correspondences.  One focal length f = (fx + fy) / 2
+// (epipolar_geometry.cpp:26-27) and thr2 = (threshold / f)^2: findEssentialMat divides the threshold by the focal length, the
+// homography works in pixels scaled by 1 / f.  Scoring: about as many CTAs in all as 4 per SM (what one pair gets on its own), at
+// least one per pair and at most one per 8 hypotheses, each staging its pair's points (cap x 32 B of shared memory).
+struct RansacGeom {
+  double f, cx, cy, thr2;
+  int H;
+  dim3 hyp, score;
+  size_t smem;
+};
+
+template <class Score>
+int ransac_geom(mvo_ctx *ctx, Score score, const double *K, double threshold, int cap, int n_pairs, RansacGeom *g) {
+  g->f = (K[0] + K[4]) / 2; g->cx = K[2]; g->cy = K[5];
+  g->thr2 = (threshold / g->f) * (threshold / g->f);
+  g->H = ctx->prm.epi_hypotheses;
   int per_pair = (4 * ctx->sm_count + n_pairs - 1) / n_pairs;
-  if (per_pair > (H + 7) / 8) per_pair = (H + 7) / 8;
+  if (per_pair > (g->H + 7) / 8) per_pair = (g->H + 7) / 8;
+  g->hyp = dim3((g->H + 127) / 128, n_pairs);
+  g->score = dim3(per_pair, n_pairs);
+  g->smem = (size_t)cap * 4 * sizeof(double);
+  if (g->smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g->smem));
+  return MVO_OK;
+}
+
+// hypotheses, scoring, finish and, with vote, recoverPose's cheirality vote of the essential-matrix RANSAC
+int epi_essential_enqueue(mvo_ctx *ctx, const RansacRows &r, int cap, int n_pairs, const double *K, double threshold, bool vote, RansacGeom *g) {
+  MVO_TRY(ransac_geom(ctx, k_epi_score_batch, K, threshold, cap, n_pairs, g));
+  const EpiCam cam = {g->f, g->cx, g->cy};
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_hypotheses_batch<<<g->hyp, 128, 0, ctx->stream>>>(r.p1, r.p2, r.pn, cap, cam, ctx->prm.pnp_seed, g->H, r.models, r.valid); }
+  MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_EPI_SCORE);
-  k_epi_score_batch<<<dim3(per_pair, n_pairs), 256, smem, ctx->stream>>>(b.p1, b.p2, b.pn, cap, cam, thr2, H, b.Es, b.valid, b.cnt); }
+  k_epi_score_batch<<<g->score, 256, g->smem, ctx->stream>>>(r.p1, r.p2, r.pn, cap, cam, g->thr2, g->H, r.models, r.valid, r.cnt); }
   MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(EpiFinSmem), k_epi_finish_batch, (const float *)b.p1, (const float *)b.p2,
-                                        (const int32_t *)b.pn, cap, cam, thr2, H, (const double *)b.Es, (const int32_t *)b.cnt, b.od, b.oi, inl)); }
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(EpiFinSmem), k_epi_finish_batch, (const float *)r.p1, (const float *)r.p2,
+                                        (const int32_t *)r.pn, cap, cam, g->thr2, g->H, (const double *)r.models, (const int32_t *)r.cnt, r.od, r.oi, r.inl)); }
   MVO_CHECK_LAUNCH(ctx);
+  if (vote) {
+    KTimer kt(ctx, KC_EPI);
+    k_epi_vote_batch<<<dim3((cap + 63) / 64, n_pairs), 256, 0, ctx->stream>>>(r.p1, r.p2, r.pn, cap, cam, r.od, r.oi, r.inl);
+    MVO_CHECK_LAUNCH(ctx);
+  }
+  return MVO_OK;
+}
+
+// hypotheses (which also zero each pair's finish outputs), scoring and finish of the homography RANSAC
+int epi_homography_enqueue(mvo_ctx *ctx, const RansacRows &r, int cap, int n_pairs, const double *K, double threshold, RansacGeom *g) {
+  MVO_TRY(ransac_geom(ctx, k_homo_score_batch, K, threshold, cap, n_pairs, g));
+  const HomoCam cam = {g->f, g->cx, g->cy};
   { KTimer kt(ctx, KC_EPI);
-  k_epi_vote_batch<<<dim3((cap + 63) / 64, n_pairs), 256, 0, ctx->stream>>>(b.p1, b.p2, b.pn, cap, cam, b.od, b.oi, inl); }
+  k_homo_hypotheses_batch<<<g->hyp, 128, 0, ctx->stream>>>(r.p1, r.p2, r.pn, cap, cam, ctx->prm.pnp_seed, g->H, r.models, r.valid, r.od, r.oi); }
   MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI_SCORE);
+  k_homo_score_batch<<<g->score, 256, g->smem, ctx->stream>>>(r.p1, r.p2, r.pn, cap, cam, g->thr2, g->H, r.models, r.valid, r.cnt); }
+  MVO_CHECK_LAUNCH(ctx);
+  { KTimer kt(ctx, KC_EPI_FINISH);
+    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(HomoFinSmem), k_homo_finish_batch, (const float *)r.p1, (const float *)r.p2,
+                                        (const int32_t *)r.pn, cap, cam, g->thr2, g->H, (const double *)r.models, (const int32_t *)r.cnt, r.od, r.oi, r.inl)); }
+  MVO_CHECK_LAUNCH(ctx);
+  return MVO_OK;
+}
+
+// The scratch of both batch calls in ctx->epib_buf, for n_pairs pairs of at most cap correspondences: the gathered pixel points
+// (with tri also the normalised-plane points), pn, the hypothesis rows (80 B per hypothesis) and the essential finish outputs.  With
+// rel (mvo_estimate_relative_poses_batch_dev; tri must be set too) also the homography finish outputs, the internal essential
+// records, both inlier rows and the (R | t) of every solution.  The homography rows reuse the hypothesis rows, which
+// k_epi_finish_batch has consumed by the time k_homo_hypotheses_batch runs on the same stream.  e.inl is left to the caller
+// unless rel.
+struct EpiBatchScratch {
+  RansacRows e, h;
+  float *np1, *np2;
+  mvo_two_view_result *ess;
+  double *rt;
+};
+
+int epi_batch_scratch(mvo_ctx *ctx, int n_pairs, int cap, bool tri, bool rel, EpiBatchScratch *b) {
+  const size_t np = (size_t)n_pairs, H = (size_t)ctx->prm.epi_hypotheses, pts = np * cap * 8, idx = np * cap * 4;
+  size_t end = 0;
+  auto take = [&end](size_t bytes) { const size_t at = end; end = (end + bytes + 255) & ~(size_t)255; return at; };
+  const size_t o_p1 = take(pts), o_p2 = take(pts), o_n1 = tri ? take(pts) : 0, o_n2 = tri ? take(pts) : 0, o_pn = take(np * 4);
+  const size_t o_E = take(np * H * 72), o_valid = take(np * H * 4), o_cnt = take(np * H * 4);
+  const size_t o_od = take(np * EPIB_OUT_D * 8), o_oi = take(np * EPIB_OUT_I * 4);
+  size_t o_hd = 0, o_hi = 0, o_ess = 0, o_ie = 0, o_ih = 0, o_rt = 0;
+  if (rel) {
+    o_hd = take(np * EPIB_OUT_D * 8); o_hi = take(np * EPIB_OUT_I * 4); o_ess = take(np * sizeof(mvo_two_view_result));
+    o_ie = take(idx); o_ih = take(idx); o_rt = take(np * 5 * 12 * 8);
+  }
+  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, end));
+  uint8_t *d = (uint8_t *)ctx->epib_buf.p;
+  *b = EpiBatchScratch();
+  RansacRows &e = b->e;
+  e.p1 = (float *)(d + o_p1); e.p2 = (float *)(d + o_p2); e.pn = (int32_t *)(d + o_pn);
+  e.models = (double *)(d + o_E); e.valid = (int32_t *)(d + o_valid); e.cnt = (int32_t *)(d + o_cnt);
+  e.od = (double *)(d + o_od); e.oi = (int32_t *)(d + o_oi);
+  if (tri) { b->np1 = (float *)(d + o_n1); b->np2 = (float *)(d + o_n2); }
+  if (rel) {
+    e.inl = (int32_t *)(d + o_ie);
+    b->h = e;
+    b->h.od = (double *)(d + o_hd); b->h.oi = (int32_t *)(d + o_hi); b->h.inl = (int32_t *)(d + o_ih);
+    b->ess = (mvo_two_view_result *)(d + o_ess); b->rt = (double *)(d + o_rt);
+  }
+  return MVO_OK;
+}
+
+// gather, the essential RANSAC with its vote, pick: six launches; pair p's inliers at b.e.inl + p * cap, its record in res[p]
+int epi_essential_batch_enqueue(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap, const int32_t *d_pairs,
+                                int n_pairs, const mvo_dmatch *d_matches, const int32_t *d_n_matches, const double *K, double threshold,
+                                const EpiBatchScratch &b, mvo_two_view_result *res) {
   { KTimer kt(ctx, KC_EPI);
-  k_epi_pick<<<(n_pairs + 127) / 128, 128, 0, ctx->stream>>>(b.pn, n_pairs, b.od, b.oi, res); }
+  k_epi_gather<<<n_pairs, 256, 0, ctx->stream>>>(d_kpts, d_counts, batch, cap, (const int2 *)d_pairs, d_matches, d_n_matches, K[0], K[4], K[2], K[5],
+                                                 b.e.p1, b.e.p2, b.np1, b.np2, b.e.pn); }
+  MVO_CHECK_LAUNCH(ctx);
+  RansacGeom g;
+  MVO_TRY(epi_essential_enqueue(ctx, b.e, cap, n_pairs, K, threshold, true, &g));
+  { KTimer kt(ctx, KC_EPI);
+  k_epi_pick<<<(n_pairs + 127) / 128, 128, 0, ctx->stream>>>(b.e.pn, n_pairs, b.e.od, b.e.oi, res); }
   MVO_CHECK_LAUNCH(ctx);
   return MVO_OK;
 }
@@ -207,21 +296,12 @@ extern "C" int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_ke
   if (!(threshold > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential batch: threshold must be positive");
   MVO_TRY(epi_batch_check(ctx, "estiMotionByEssential batch", batch, cap, n_pairs, K));
   if (n_pairs == 0) return MVO_OK;
-  const int H = ctx->prm.epi_hypotheses;
   const bool tri = d_pts3d != nullptr;
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t np = (size_t)n_pairs, pts = al(np * cap * 8);
-  const size_t o_p1 = 0, o_p2 = o_p1 + pts, o_n1 = o_p2 + pts, o_n2 = o_n1 + (tri ? pts : 0), o_pn = o_n2 + (tri ? pts : 0);
-  const size_t o_E = al(o_pn + np * 4), o_valid = al(o_E + np * H * 72), o_cnt = al(o_valid + np * H * 4), o_od = al(o_cnt + np * H * 4);
-  const size_t o_oi = al(o_od + np * EPIB_OUT_D * 8), o_end = o_oi + np * EPIB_OUT_I * 4;
-  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, o_end));
-  uint8_t *d = (uint8_t *)ctx->epib_buf.p;
   EpiBatchScratch b;
-  b.p1 = (float *)(d + o_p1); b.p2 = (float *)(d + o_p2); b.np1 = tri ? (float *)(d + o_n1) : nullptr; b.np2 = tri ? (float *)(d + o_n2) : nullptr;
-  b.pn = (int32_t *)(d + o_pn); b.valid = (int32_t *)(d + o_valid); b.cnt = (int32_t *)(d + o_cnt); b.oi = (int32_t *)(d + o_oi);
-  b.Es = (double *)(d + o_E); b.od = (double *)(d + o_od);
-  MVO_TRY(epi_essential_batch_enqueue(ctx, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K, threshold, b, d_res, d_inliers));
+  MVO_TRY(epi_batch_scratch(ctx, n_pairs, cap, tri, false, &b));
+  b.e.inl = d_inliers;
+  MVO_TRY(epi_essential_batch_enqueue(ctx, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K, threshold, b, d_res));
   if (tri) {
     KTimer kt(ctx, KC_EPI);
     k_triangulate_batch<<<dim3((cap + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(b.np1, b.np2, d_res, cap, d_inliers, d_pts3d);
@@ -236,9 +316,7 @@ int mvo_relative_poses_combine(mvo_ctx *ctx, const MvoRelPosesCombine &a) __attr
 
 // mvo_estimate_relative_poses_batch_dev (mvo.h): the essential half (six launches, into an internal mvo_two_view_result array),
 // the homography half (three launches), the combine step (two_view_batch.cu: decomposition, visibility filter, inlier rows,
-// invRt, scores, E/H choice) and, with d_pts3d, one triangulation launch over (pair, solution).  Scratch in ctx->epib_buf: the
-// homography half reuses the essential half's hypothesis rows (80 B per hypothesis), which k_epi_finish_batch has consumed by the
-// time k_homo_hypotheses_batch runs on the same stream.
+// invRt, scores, E/H choice) and, with d_pts3d, one triangulation launch over (pair, solution).  Scratch in ctx->epib_buf.
 extern "C" int mvo_estimate_relative_poses_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
                                                      const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
                                                      const int32_t *d_n_matches, const double *K, int motion_cam2_to_cam1,
@@ -252,58 +330,28 @@ extern "C" int mvo_estimate_relative_poses_batch_dev(mvo_ctx *ctx, const mvo_key
   double Ki[9];
   if (!epi::inv3(K, Ki)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: singular (checkEssentialScore inverts it)");
   if (n_pairs == 0) return MVO_OK;
-  const int H = ctx->prm.epi_hypotheses;
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t np = (size_t)n_pairs, pts = al(np * cap * 8), idx = al(np * cap * 4);
-  const size_t o_p1 = 0, o_p2 = o_p1 + pts, o_n1 = o_p2 + pts, o_n2 = o_n1 + pts, o_pn = o_n2 + pts;
-  const size_t o_E = al(o_pn + np * 4), o_valid = al(o_E + np * H * 72), o_cnt = al(o_valid + np * H * 4), o_od = al(o_cnt + np * H * 4);
-  const size_t o_oi = al(o_od + np * EPIB_OUT_D * 8), o_hd = al(o_oi + np * EPIB_OUT_I * 4), o_hi = al(o_hd + np * EPIB_OUT_D * 8);
-  const size_t o_ess = al(o_hi + np * EPIB_OUT_I * 4), o_ie = al(o_ess + np * sizeof(mvo_two_view_result)), o_ih = o_ie + idx;
-  const size_t o_rt = o_ih + idx, o_end = o_rt + np * 5 * 12 * 8;
-  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, o_end));
-  uint8_t *d = (uint8_t *)ctx->epib_buf.p;
   EpiBatchScratch b;
-  b.p1 = (float *)(d + o_p1); b.p2 = (float *)(d + o_p2); b.np1 = (float *)(d + o_n1); b.np2 = (float *)(d + o_n2);
-  b.pn = (int32_t *)(d + o_pn); b.valid = (int32_t *)(d + o_valid); b.cnt = (int32_t *)(d + o_cnt); b.oi = (int32_t *)(d + o_oi);
-  b.Es = (double *)(d + o_E); b.od = (double *)(d + o_od);
-  mvo_two_view_result *ess = (mvo_two_view_result *)(d + o_ess);
-  int32_t *inl_e = (int32_t *)(d + o_ie), *inl_h = (int32_t *)(d + o_ih), *hoi = (int32_t *)(d + o_hi);
-  double *hod = (double *)(d + o_hd), *rt = (double *)(d + o_rt);
+  MVO_TRY(epi_batch_scratch(ctx, n_pairs, cap, true, true, &b));
   // ---- essential half (:43-48) ----
   MVO_TRY(epi_essential_batch_enqueue(ctx, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, K, ctx->prm.essential_threshold,
-                                      b, ess, inl_e));
-  // ---- homography half (:56-67), as mvo_epi_homography_begin on the same points ----
-  HomoCam hc;
-  hc.f = (K[0] + K[4]) / 2; hc.cx = K[2]; hc.cy = K[5];
-  const double hthr2 = (ctx->prm.homography_threshold / hc.f) * (ctx->prm.homography_threshold / hc.f);
-  const size_t smem = (size_t)cap * 4 * sizeof(double);
-  { KTimer kt(ctx, KC_EPI);
-  k_homo_hypotheses_batch<<<dim3((H + 127) / 128, n_pairs), 128, 0, ctx->stream>>>(b.p1, b.p2, b.pn, cap, hc, ctx->prm.pnp_seed, H, b.Es, b.valid, hod, hoi); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_homo_score_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_pair = (4 * ctx->sm_count + n_pairs - 1) / n_pairs;
-  if (per_pair > (H + 7) / 8) per_pair = (H + 7) / 8;
-  { KTimer kt(ctx, KC_EPI_SCORE);
-  k_homo_score_batch<<<dim3(per_pair, n_pairs), 256, smem, ctx->stream>>>(b.p1, b.p2, b.pn, cap, hc, hthr2, H, b.Es, b.valid, b.cnt); }
-  MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, (unsigned)n_pairs, sizeof(HomoFinSmem), k_homo_finish_batch, (const float *)b.p1, (const float *)b.p2,
-                                        (const int32_t *)b.pn, cap, hc, hthr2, H, (const double *)b.Es, (const int32_t *)b.cnt, hod, hoi, inl_h)); }
-  MVO_CHECK_LAUNCH(ctx);
+                                      b, b.ess));
+  // ---- homography half (:56-67), on the same points ----
+  RansacGeom g;
+  MVO_TRY(epi_homography_enqueue(ctx, b.h, cap, n_pairs, K, ctx->prm.homography_threshold, &g));
   // ---- combine (:56-154 after the RANSACs) ----
   MvoRelPosesCombine a;
-  a.n_matches = d_n_matches; a.ess = ess; a.inl_e = inl_e; a.hom_i = hoi; a.inl_h = inl_h; a.hom_d = hod;
-  a.p1 = b.p1; a.p2 = b.p2; a.np1 = b.np1; a.np2 = b.np2;
+  a.n_matches = d_n_matches; a.ess = b.ess; a.inl_e = b.e.inl; a.hom_i = b.h.oi; a.inl_h = b.h.inl; a.hom_d = b.h.od;
+  a.p1 = b.e.p1; a.p2 = b.e.p2; a.np1 = b.np1; a.np2 = b.np2;
   a.n_pairs = n_pairs; a.cap = cap; a.hom_d_stride = EPIB_OUT_D; a.hom_i_stride = EPIB_OUT_I; a.motion_cam2_to_cam1 = motion_cam2_to_cam1;
   for (int q = 0; q < 9; ++q) a.K[q] = K[q];
   a.eh_ratio_threshold = ctx->prm.eh_ratio_threshold;
-  a.res = d_res; a.inliers = d_inliers; a.rt = rt;
+  a.res = d_res; a.inliers = d_inliers; a.rt = b.rt;
   MVO_TRY(mvo_relative_poses_combine(ctx, a));
   // ---- triangulation of every solution (:105-112), with the (R, t) from before invRt ----
   if (d_pts3d) {
     KTimer kt(ctx, KC_EPI);
-    k_triangulate_solutions_batch<<<dim3((cap + 127) / 128, 5, n_pairs), 128, 0, ctx->stream>>>(b.np1, b.np2, d_res, rt, cap, d_inliers, d_pts3d);
+    k_triangulate_solutions_batch<<<dim3((cap + 127) / 128, 5, n_pairs), 128, 0, ctx->stream>>>(b.np1, b.np2, d_res, b.rt, cap, d_inliers, d_pts3d);
     MVO_CHECK_LAUNCH(ctx);
   }
   return MVO_OK;
@@ -318,28 +366,28 @@ int mvo_epi_essential_begin(mvo_ctx *ctx, const float *pts1, const float *pts2, 
   if (!pts1 || !pts2 || !K || !job) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential: null pointer");
   if (n < 8) return mvo_fail(ctx, MVO_ERR_DEGENERATE, "estiMotionByEssential: %d correspondences (< 8)", n);
   if (!(threshold > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByEssential: threshold must be positive");
-  EpiCam cam;
-  cam.f = (K[0] + K[4]) / 2; cam.cx = K[2]; cam.cy = K[5];               // epipolar_geometry.cpp:26-27
-  if (!(cam.f > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal length must be positive");
-  const size_t smem = (size_t)n * 4 * sizeof(double);
-  if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential: more than %d correspondences", 200 * 1024 / 32);
+  if (!((K[0] + K[4]) / 2 > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal length must be positive");
+  if ((size_t)n * 4 * sizeof(double) > 200 * 1024)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential: more than %d correspondences", 200 * 1024 / 32);
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
   const int H = ctx->prm.epi_hypotheses;
   auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t o_p1 = 0, o_p2 = al(o_p1 + (size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8), o_E = al(o_inl + (size_t)n * 4);
+  // a batch of one: pn[0] = n follows p2 in the same copy
+  const size_t o_p1 = 0, o_p2 = al(o_p1 + (size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8 + 4), o_E = al(o_inl + (size_t)n * 4);
   const size_t o_valid = al(o_E + (size_t)H * 72), o_cnt = al(o_valid + (size_t)H * 4), o_out = al(o_cnt + (size_t)H * 4);
   // optional triangulation block: np1, np2 (n x 2 floats each), R | t (12 doubles), out (n x 3 floats)
   const size_t o_t1 = al(o_out + 512), o_t2 = al(o_t1 + (size_t)n * 8), o_trt = al(o_t2 + (size_t)n * 8), o_tout = al(o_trt + 96);
   const size_t o_end = tri ? o_tout + (size_t)n * 12 : o_out + 512;
-  // pinned staging: [p1 p2 | np1 np2 Rt] in, [out block 512 B + inliers | triangulated points] out
-  const size_t h_in = al((size_t)n * 16) + (tri ? al((size_t)n * 16) + 256 : 0), h_res = 512 + al((size_t)n * 4) + 256;
+  // pinned staging: [p1 p2 pn | np1 np2 Rt] in, [out block 512 B + inliers | triangulated points] out
+  const size_t h_in = al((size_t)n * 16 + 4) + (tri ? al((size_t)n * 16) + 256 : 0), h_res = 512 + al((size_t)n * 4) + 256;
   MVO_TRY(mvo_reserve(ctx, ctx->d_a, o_end));
   MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_a, h_in + h_res + (tri ? (size_t)n * 12 : 0) + 1024));
   uint8_t *d = (uint8_t *)ctx->d_a.p, *h = (uint8_t *)ctx->h_a.p;
   memcpy(h, pts1, (size_t)n * 8);
   memcpy(h + (size_t)n * 8, pts2, (size_t)n * 8);
+  memcpy(h + (size_t)n * 16, &n, 4);
   MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p1, h, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p2, h + (size_t)n * 8, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p2, h + (size_t)n * 8, (size_t)n * 8 + 4, cudaMemcpyHostToDevice, ctx->stream));
   // the triangulation does not depend on the RANSAC: it runs on the context's side stream next to it (on the same stream when
   // per-kernel event timing is on, or when this job itself was pointed at the side stream)
   cudaStream_t tri_stream = ctx->stream;
@@ -347,7 +395,7 @@ int mvo_epi_essential_begin(mvo_ctx *ctx, const float *pts1, const float *pts2, 
   if (tri) {
     cudaStream_t side = ctx->timing_mask ? nullptr : mvo_side_stream(ctx);
     if (side && side != ctx->stream) tri_stream = side;
-    uint8_t *ht = h + al((size_t)n * 16);
+    uint8_t *ht = h + al((size_t)n * 16 + 4);
     memcpy(ht, tri_np1, (size_t)n * 8);
     memcpy(ht + (size_t)n * 8, tri_np2, (size_t)n * 8);
     memcpy(ht + al((size_t)n * 16), tri_R, 72);
@@ -366,34 +414,19 @@ int mvo_epi_essential_begin(mvo_ctx *ctx, const float *pts1, const float *pts2, 
     MVO_CHECK_LAUNCH(ctx);
     MVO_CUDA(ctx, cudaMemcpyAsync(h_tri, d + o_tout, (size_t)n * 12, cudaMemcpyDeviceToHost, tri_stream));
   }
-  const float *d1 = (const float *)(d + o_p1), *d2 = (const float *)(d + o_p2);
-  double *dE = (double *)(d + o_E), *dout = (double *)(d + o_out);
-  int32_t *dvalid = (int32_t *)(d + o_valid), *dcnt = (int32_t *)(d + o_cnt), *dinl = (int32_t *)(d + o_inl), *dout_i = (int32_t *)(d + o_out + 256);
-  const double thr2 = (threshold / cam.f) * (threshold / cam.f);          // findEssentialMat: threshold /= focal
-  { KTimer kt(ctx, KC_EPI);
-  k_epi_hypotheses<<<(H + 127) / 128, 128, 0, ctx->stream>>>(d1, d2, n, cam, ctx->prm.pnp_seed, H, dE, dvalid); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_epi_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int grid = (H + 7) / 8;
-  if (grid > 4 * ctx->sm_count) grid = 4 * ctx->sm_count;
-  { KTimer kt(ctx, KC_EPI_SCORE);
-  k_epi_score<<<grid, 256, smem, ctx->stream>>>(d1, d2, n, cam, thr2, H, dE, dvalid, dcnt); }
-  MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, 1, sizeof(EpiFinSmem), k_epi_finish, d1, d2, n, cam, thr2, H, (const double *)dE, (const int32_t *)dcnt, dout, dout_i, dinl)); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (want_pose) {
-    KTimer kt(ctx, KC_EPI);
-    k_epi_vote<<<(n + 63) / 64, 256, 0, ctx->stream>>>(d1, d2, cam, dout, dout_i, dinl);
-    MVO_CHECK_LAUNCH(ctx);
-  }
+  RansacRows r;
+  r.p1 = (float *)(d + o_p1); r.p2 = (float *)(d + o_p2); r.pn = (int32_t *)(d + o_p2 + (size_t)n * 8);
+  r.models = (double *)(d + o_E); r.valid = (int32_t *)(d + o_valid); r.cnt = (int32_t *)(d + o_cnt);
+  r.od = (double *)(d + o_out); r.oi = (int32_t *)(d + o_out + 256); r.inl = (int32_t *)(d + o_inl);
+  RansacGeom g;
+  MVO_TRY(epi_essential_enqueue(ctx, r, n, 1, K, threshold, want_pose != 0, &g));
   double *h_out = (double *)(h + h_in);
   int32_t *h_inl = (int32_t *)((uint8_t *)h_out + 512);
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_out, dout, 512, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_inl, dinl, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(h_out, r.od, 512, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(h_inl, r.inl, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   job->tri_stream = tri_stream;
-  job->stream = ctx->stream; job->n = n; job->H = H; job->want_pose = want_pose != 0; job->tri = tri; job->thr2 = thr2; job->f = cam.f;
-  job->h_out = h_out; job->h_inl = h_inl; job->h_tri = h_tri; job->d_valid = dvalid; job->d_cnt = dcnt; job->d_model = dE;
+  job->stream = ctx->stream; job->n = n; job->H = H; job->want_pose = want_pose != 0; job->tri = tri; job->thr2 = g.thr2; job->f = g.f;
+  job->h_out = h_out; job->h_inl = h_inl; job->h_tri = h_tri; job->d_valid = r.valid; job->d_cnt = r.cnt; job->d_model = r.models;
   return MVO_OK;
 }
 
@@ -469,46 +502,35 @@ int mvo_epi_homography_begin(mvo_ctx *ctx, const float *pts1, const float *pts2,
   if (!pts1 || !pts2 || !K || !job) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByHomography: null pointer");
   if (n < 4) return mvo_fail(ctx, MVO_ERR_DEGENERATE, "estiMotionByHomography: %d correspondences (< 4)", n);
   if (!(threshold > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByHomography: threshold must be positive");
-  HomoCam cam;
-  cam.f = (K[0] + K[4]) / 2; cam.cx = K[2]; cam.cy = K[5];
   if (!(K[0] > 0 && K[4] > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal lengths must be positive");
-  const size_t smem = (size_t)n * 4 * sizeof(double);
-  if (smem > 200 * 1024) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByHomography: more than %d correspondences", 200 * 1024 / 32);
+  if ((size_t)n * 4 * sizeof(double) > 200 * 1024)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByHomography: more than %d correspondences", 200 * 1024 / 32);
   MVO_CUDA(ctx, cudaSetDevice(ctx->device));
   const int H = ctx->prm.epi_hypotheses;
   auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t o_p1 = 0, o_p2 = al(o_p1 + (size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8), o_H = al(o_inl + (size_t)n * 4);
+  // a batch of one: pn[0] = n follows p2 in the same copy
+  const size_t o_p1 = 0, o_p2 = al(o_p1 + (size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8 + 4), o_H = al(o_inl + (size_t)n * 4);
   const size_t o_valid = al(o_H + (size_t)H * 72), o_cnt = al(o_valid + (size_t)H * 4), o_out = al(o_cnt + (size_t)H * 4), o_end = o_out + 512;
   MVO_TRY(mvo_reserve(ctx, ctx->d_e, o_end));
-  MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_c, al((size_t)n * 16) + (size_t)n * 4 + 1024));
+  MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_c, al((size_t)n * 16 + 4) + (size_t)n * 4 + 1024));
   uint8_t *d = (uint8_t *)ctx->d_e.p, *h = (uint8_t *)ctx->h_c.p;
   memcpy(h, pts1, (size_t)n * 8);
   memcpy(h + (size_t)n * 8, pts2, (size_t)n * 8);
+  memcpy(h + (size_t)n * 16, &n, 4);
   MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p1, h, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p2, h + (size_t)n * 8, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  const float *d1 = (const float *)(d + o_p1), *d2 = (const float *)(d + o_p2);
-  double *dH = (double *)(d + o_H), *dout = (double *)(d + o_out);
-  int32_t *dvalid = (int32_t *)(d + o_valid), *dcnt = (int32_t *)(d + o_cnt), *dinl = (int32_t *)(d + o_inl), *dout_i = (int32_t *)(d + o_out + 256);
-  const double thr2 = (threshold / cam.f) * (threshold / cam.f);          // pixels -> scaled coordinates
-  MVO_CUDA(ctx, cudaMemsetAsync(dout, 0, 512, ctx->stream));
-  { KTimer kt(ctx, KC_EPI);
-  k_homo_hypotheses<<<(H + 127) / 128, 128, 0, ctx->stream>>>(d1, d2, n, cam, ctx->prm.pnp_seed, H, dH, dvalid); }
-  MVO_CHECK_LAUNCH(ctx);
-  if (smem > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_homo_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int grid = (H + 7) / 8;
-  if (grid > 4 * ctx->sm_count) grid = 4 * ctx->sm_count;
-  { KTimer kt(ctx, KC_EPI_SCORE);
-  k_homo_score<<<grid, 256, smem, ctx->stream>>>(d1, d2, n, cam, thr2, H, dH, dvalid, dcnt); }
-  MVO_CHECK_LAUNCH(ctx);
-  { KTimer kt(ctx, KC_EPI_FINISH);
-    MVO_CUDA(ctx, launch_finish_cluster(ctx, 1, sizeof(HomoFinSmem), k_homo_finish, d1, d2, n, cam, thr2, H, (const double *)dH, (const int32_t *)dcnt, dout, dout_i, dinl)); }
-  MVO_CHECK_LAUNCH(ctx);
-  double *h_out = (double *)(h + al((size_t)n * 16));
+  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p2, h + (size_t)n * 8, (size_t)n * 8 + 4, cudaMemcpyHostToDevice, ctx->stream));
+  RansacRows r;
+  r.p1 = (float *)(d + o_p1); r.p2 = (float *)(d + o_p2); r.pn = (int32_t *)(d + o_p2 + (size_t)n * 8);
+  r.models = (double *)(d + o_H); r.valid = (int32_t *)(d + o_valid); r.cnt = (int32_t *)(d + o_cnt);
+  r.od = (double *)(d + o_out); r.oi = (int32_t *)(d + o_out + 256); r.inl = (int32_t *)(d + o_inl);
+  RansacGeom g;
+  MVO_TRY(epi_homography_enqueue(ctx, r, n, 1, K, threshold, &g));
+  double *h_out = (double *)(h + al((size_t)n * 16 + 4));
   int32_t *h_inl = (int32_t *)((uint8_t *)h_out + 512);
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_out, dout, 512, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_inl, dinl, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(h_out, r.od, 512, cudaMemcpyDeviceToHost, ctx->stream));
+  MVO_CUDA(ctx, cudaMemcpyAsync(h_inl, r.inl, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   memset(job, 0, sizeof *job);
-  job->stream = ctx->stream; job->n = n; job->H = H; job->thr2 = thr2; job->f = cam.f; job->h_out = h_out; job->h_inl = h_inl;
+  job->stream = ctx->stream; job->n = n; job->H = H; job->thr2 = g.thr2; job->f = g.f; job->h_out = h_out; job->h_inl = h_inl;
   return MVO_OK;
 }
 
@@ -618,33 +640,7 @@ extern "C" {
 
 int mvo_do_triangulation(mvo_ctx *ctx, const float *pts_np1, const float *pts_np2, int n, const double *R, const double *t,
                          const int32_t *inliers, int n_inliers, float *pts3d) {
-  if (!ctx) return MVO_ERR_INVALID_ARG;
-  if (n < 0 || n_inliers < 0 || !R || !t || (n > 0 && (!pts_np1 || !pts_np2)) || (n_inliers > 0 && (!inliers || !pts3d)))
-    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "doTriangulation: null pointer");
-  for (int j = 0; j < n_inliers; ++j)
-    if (inliers[j] < 0 || inliers[j] >= n) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "doTriangulation: inlier index %d outside [0,%d)", inliers[j], n);
-  if (n_inliers == 0) return MVO_OK;
-  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t o_p1 = 0, o_p2 = al((size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8), o_rt = al(o_inl + (size_t)n_inliers * 4);
-  const size_t o_out = al(o_rt + 96), o_end = o_out + (size_t)n_inliers * 12;
-  MVO_TRY(mvo_reserve(ctx, ctx->d_b, o_end + 256));
-  MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_a, o_end + 256));
-  uint8_t *d = (uint8_t *)ctx->d_b.p, *h = (uint8_t *)ctx->h_a.p;
-  memcpy(h + o_p1, pts_np1, (size_t)n * 8);
-  memcpy(h + o_p2, pts_np2, (size_t)n * 8);
-  memcpy(h + o_inl, inliers, (size_t)n_inliers * 4);
-  memcpy(h + o_rt, R, 72);
-  memcpy(h + o_rt + 72, t, 24);
-  MVO_CUDA(ctx, cudaMemcpyAsync(d, h, o_out, cudaMemcpyHostToDevice, ctx->stream));
-  { KTimer kt(ctx, KC_EPI);
-  k_triangulate<<<(n_inliers + 127) / 128, 128, 0, ctx->stream>>>((const float *)(d + o_p1), (const float *)(d + o_p2), (const int32_t *)(d + o_inl),
-                                                                  n_inliers, (const double *)(d + o_rt), (float *)(d + o_out)); }
-  MVO_CHECK_LAUNCH(ctx);
-  MVO_CUDA(ctx, cudaMemcpyAsync(h + o_out, d + o_out, (size_t)n_inliers * 12, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  memcpy(pts3d, h + o_out, (size_t)n_inliers * 12);
-  return MVO_OK;
+  return mvo_do_triangulation_multi(ctx, pts_np1, pts_np2, n, 1, &R, &t, &inliers, &n_inliers, &pts3d);
 }
 
 }  // extern "C"

@@ -13,9 +13,8 @@ __device__ __forceinline__ uint64_t splitmix64e(uint64_t x) {
 
 struct EpiCam { double f, cx, cy; };      // findEssentialMat(focal, pp): one focal length (epipolar_geometry.cpp:26-27)
 
-// The kernel bodies below are device functions that the single-pair kernels and their batched counterparts (one pair per
-// blockIdx.y, or one cluster per pair for the finish; mvo_esti_motion_by_essential_batch_dev) both call: the arithmetic exists
-// once, so a pair of a batch gets the bits of a single call on the same points.
+// The kernel bodies below are device functions of one pair; the kernels of the batch sections run them for every pair (one pair
+// per blockIdx.y, or one cluster per pair for the finish).  A single-pair call is a batch of one (epipolar.cu).
 
 // hypothesis h: counter-based minimal sample of 8 distinct correspondences, epi::essential_from_8
 __device__ __forceinline__ void epi_hypothesis(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, uint64_t seed,
@@ -44,14 +43,6 @@ __device__ __forceinline__ void epi_hypothesis(const float *__restrict__ p1, con
   valid[h] = ok ? 1 : -reason;             // <= 0: rejected sample (the reason is kept for MVO_EPI_DEBUG)
 }
 
-__global__ void __launch_bounds__(128)
-k_epi_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, uint64_t seed, int H,
-                 double *__restrict__ Es, int32_t *__restrict__ valid) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= H) return;
-  epi_hypothesis(p1, p2, n, cam, seed, h, Es, valid);
-}
-
 // Sampson consensus of hypotheses cta * warps + warp, strided by ncta * warps; the CTA stages the n points once
 __device__ __forceinline__ void epi_score_run(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
                                               const double *__restrict__ Es, const int32_t *__restrict__ valid, int32_t *__restrict__ counts,
@@ -73,12 +64,6 @@ __device__ __forceinline__ void epi_score_run(const float *__restrict__ p1, cons
     for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
     if (lane == 0) counts[h] = c;
   }
-}
-
-__global__ void __launch_bounds__(256)
-k_epi_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
-            const double *__restrict__ Es, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
-  epi_score_run(p1, p2, n, cam, thr2, H, Es, valid, counts, blockIdx.x, gridDim.x);
 }
 
 constexpr int EFIN_T = 256;       // 255 registers per thread: the 20 (54) Gauss-Newton accumulators stay in registers (1024 threads = 64 registers spilled them)
@@ -110,7 +95,7 @@ __device__ __forceinline__ void so3_exp(const double *w, double *R) {
   R[6] = -A * y + B * x * z;      R[7] = A * x + B * y * z;       R[8] = 1 - B * (x * x + y * y);
 }
 
-// The estimate the Gauss-Newton iteration of k_epi_finish moves: R, the unit translation t and an orthonormal basis (b1, b2) of
+// The estimate the Gauss-Newton iteration of epi_finish_run moves: R, the unit translation t and an orthonormal basis (b1, b2) of
 // the tangent plane of the unit sphere at t.  A step d = (rotation increment on the right, two tangent-plane components).
 struct EpiPose { double R[9], t[3], b1[3], b2[3]; };
 
@@ -209,7 +194,7 @@ __device__ __forceinline__ double sampson_signed(const double *E, double x1, dou
 
 // out_d: [0..8] E (scaled so that E[8] = 1, epipolar_geometry.cpp:37), [9..17] R1, [18..26] R2, [27..29] t of
 // decomposeEssentialMat; out_i: [0] inliers, [1] best hypothesis, [3] consensus of the best minimal model, [4] consensus after the
-// local optimisation, [5] Gauss-Newton iterations run, [8..11] cheirality votes (k_epi_vote)
+// local optimisation, [5] Gauss-Newton iterations run, [8..11] cheirality votes (k_epi_vote_batch)
 //
 // After the arg-max the best minimal model is locally optimised (LO-RANSAC style): EPI_LO_ROUNDS times its consensus
 // set is re-selected and (R, t/|t|) is re-estimated on it by Gauss-Newton on the signed Sampson residual (5 degrees of
@@ -410,7 +395,7 @@ __device__ __forceinline__ void epi_finish_run(const float *__restrict__ p1, con
     if (r < rank) off += c;
     n_in += c;
   }
-  // the consensus set, ascending; the cheirality vote of recoverPose runs in k_epi_vote (all SMs) and the host picks
+  // the consensus set, ascending; the cheirality vote of recoverPose runs in k_epi_vote_batch (all SMs), the pick on the host or in k_epi_pick
   for (int i = b0; i < e0; ++i) {
     const double x1 = ((double)p1[2 * i] - cam.cx) / cam.f, y1 = ((double)p1[2 * i + 1] - cam.cy) / cam.f;
     const double x2 = ((double)p2[2 * i] - cam.cx) / cam.f, y2 = ((double)p2[2 * i + 1] - cam.cy) / cam.f;
@@ -421,16 +406,9 @@ __device__ __forceinline__ void epi_finish_run(const float *__restrict__ p1, con
     for (int q = 0; q < 9; ++q) { out_d[q] = S.E[q] / e22; out_d[9 + q] = S.R1[q]; out_d[18 + q] = S.R2[q]; }       // E /= E(2,2) (:37)
     for (int q = 0; q < 3; ++q) out_d[27 + q] = S.t[q];
     out_i[0] = n_in; out_i[1] = S.best;
-    out_i[8] = out_i[9] = out_i[10] = out_i[11] = 0;                      // votes, accumulated by k_epi_vote
+    out_i[8] = out_i[9] = out_i[10] = out_i[11] = 0;                      // votes, accumulated by k_epi_vote_batch
   }
   cluster.sync();                                    // no CTA leaves while another still reads its shared memory
-}
-
-__global__ void __launch_bounds__(EFIN_T)
-k_epi_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, EpiCam cam, double thr2, int H,
-             const double *__restrict__ Es, const int32_t *__restrict__ counts, double *__restrict__ out_d,
-             int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
-  epi_finish_run(p1, p2, n, cam, thr2, H, Es, counts, out_d, out_i, inl);
 }
 
 // recoverPose (calib3d five-point.cpp): triangulate every inlier with [I|0] and each of (R1,t) (R2,t) (R1,-t) (R2,-t); a point
@@ -465,12 +443,6 @@ __device__ __forceinline__ void epi_vote_run(const float *__restrict__ p1, const
   }
 }
 
-__global__ void __launch_bounds__(256)
-k_epi_vote(const float *__restrict__ p1, const float *__restrict__ p2, EpiCam cam, const double *__restrict__ out_d,
-           int32_t *__restrict__ out_i, const int32_t *__restrict__ inl) {
-  epi_vote_run(p1, p2, cam, out_d, out_i, inl, blockIdx.x);
-}
-
 // doTriangulation of correspondence i into row j of out
 __device__ __forceinline__ void epi_triangulate_one(const float *__restrict__ np1, const float *__restrict__ np2, int i,
                                                     const double *__restrict__ Rt /* 9 + 3 */, float *__restrict__ out, int j) {
@@ -494,9 +466,10 @@ k_triangulate(const float *__restrict__ np1, const float *__restrict__ np2, cons
 }
 
 // ------------------------------------------------------------------------------------ batch of frame pairs
-// mvo_esti_motion_by_essential_batch_dev: the kernels above for n_pairs matched frame pairs at once.  Pair p's scratch rows:
-// points at p * cap, hypotheses at p * H, finish outputs at p * EPIB_OUT_D / p * EPIB_OUT_I.  pn[p] (written by k_epi_gather):
-// the pair's correspondence count, or MVO_ERR_INVALID_ARG; every later kernel skips a pair whose pn is below 8.
+// The essential-matrix kernels for n_pairs matched frame pairs at once (a single-pair call: one pair, cap = n).  Pair p's scratch
+// rows: points at p * cap, hypotheses at p * H, finish outputs at p * EPIB_OUT_D / p * EPIB_OUT_I.  pn[p] (written by k_epi_gather,
+// or uploaded with the points): the pair's correspondence count, or MVO_ERR_INVALID_ARG; every later kernel skips a pair whose pn
+// is below 8.
 constexpr int EPIB_OUT_D = 32, EPIB_OUT_I = 16;
 
 // One CTA per pair: checks the frame indices, the match count and every match's keypoint indices before reading through them,
@@ -548,7 +521,7 @@ k_epi_score_batch(const float *__restrict__ p1, const float *__restrict__ p2, co
   epi_score_run(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, thr2, H, Es + oh * 9, valid + oh, counts + oh, blockIdx.x, gridDim.x);
 }
 
-// one cluster per pair: CTAs [pair * csize, (pair + 1) * csize) along x, the cluster size and rank split of k_epi_finish
+// one cluster per pair: CTAs [pair * csize, (pair + 1) * csize) along x
 __global__ void __launch_bounds__(EFIN_T)
 k_epi_finish_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, EpiCam cam, double thr2,
                    int H, const double *__restrict__ Es, const int32_t *__restrict__ counts, double *__restrict__ out_d,
@@ -648,14 +621,6 @@ __device__ __forceinline__ void homo_hypothesis(const float *__restrict__ p1, co
   valid[h] = ok ? 1 : 0;
 }
 
-__global__ void __launch_bounds__(128)
-k_homo_hypotheses(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, uint64_t seed, int H,
-                  double *__restrict__ Hs, int32_t *__restrict__ valid) {
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= H) return;
-  homo_hypothesis(p1, p2, n, cam, seed, h, Hs, valid);
-}
-
 // forward transfer error consensus of hypotheses cta * warps + warp, strided by ncta * warps; the CTA stages the n points once
 __device__ __forceinline__ void homo_score_run(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
                                                const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts,
@@ -677,12 +642,6 @@ __device__ __forceinline__ void homo_score_run(const float *__restrict__ p1, con
     for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
     if (lane == 0) counts[h] = c;
   }
-}
-
-__global__ void __launch_bounds__(256)
-k_homo_score(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
-             const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
-  homo_score_run(p1, p2, n, cam, thr2, H, Hs, valid, counts, blockIdx.x, gridDim.x);
 }
 
 constexpr int HOMO_NV = epi::HOMO_GN_NV;    // 45 entries of J^T J (upper triangle) + 9 of J^T r
@@ -758,7 +717,7 @@ __device__ __forceinline__ bool homography_gn_step_warp(const double *sum, doubl
 
 // out_d: [0..8] H in pixel coordinates scaled so that H[8] = 1; out_i: [0] inliers, [1] best hypothesis,
 // [3] consensus of the best minimal model, [4] consensus after the local optimisation, [5] Gauss-Newton iterations run
-// One cluster of EFIN_C CTAs like k_epi_finish: every CTA owns a slice of the correspondences, the partial normal equations are
+// One cluster of EFIN_C CTAs like epi_finish_run: every CTA owns a slice of the correspondences, the partial normal equations are
 // summed in rank order through distributed shared memory (bit-identical in every CTA), thread 0 of every CTA takes the step.
 struct HomoFinSmem {
   long long k[EFIN_T / 32];
@@ -914,18 +873,12 @@ __device__ __forceinline__ void homo_finish_run(const float *__restrict__ p1, co
   cluster.sync();                                    // no CTA leaves while another still reads its shared memory
 }
 
-__global__ void __launch_bounds__(EFIN_T, 1)
-k_homo_finish(const float *__restrict__ p1, const float *__restrict__ p2, int n, HomoCam cam, double thr2, int H,
-              const double *__restrict__ Hs, const int32_t *__restrict__ counts, double *__restrict__ out_d,
-              int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
-  homo_finish_run(p1, p2, n, cam, thr2, H, Hs, counts, out_d, out_i, inl);
-}
-
 // ------------------------------------------------------------------------- homography for a batch of frame pairs
-// mvo_estimate_relative_poses_batch_dev: the three homography kernels over the pairs of the essential batch (same pn, same
-// point rows; the hypotheses reuse the essential half's hypothesis rows, which are free once k_epi_finish_batch has run).
-// Pair p's finish outputs at p * EPIB_OUT_D / p * EPIB_OUT_I: the single call zeroes its 512-byte output block before the
-// launches, k_homo_hypotheses_batch does it here (CTA 0 of each pair), so a pair without any model reads 0 inliers.
+// The three homography kernels over the pairs of the essential batch (same pn, same point rows; in
+// mvo_estimate_relative_poses_batch_dev the hypotheses reuse the essential half's hypothesis rows, which are free once
+// k_epi_finish_batch has run), or over the one pair of a single call.  Pair p's finish outputs at p * EPIB_OUT_D / p * EPIB_OUT_I:
+// k_homo_hypotheses_batch zeroes them (CTA 0 of each pair), so a pair without any model reads 0 inliers.  A pair is skipped below
+// 4 correspondences, the minimal sample (a single call accepts 4 to 7; in a batch such a pair fails in the essential half).
 __global__ void __launch_bounds__(128)
 k_homo_hypotheses_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, HomoCam cam,
                         uint64_t seed, int H, double *__restrict__ Hs, int32_t *__restrict__ valid, double *__restrict__ out_d,
@@ -935,7 +888,7 @@ k_homo_hypotheses_batch(const float *__restrict__ p1, const float *__restrict__ 
     out_d[(size_t)pair * EPIB_OUT_D + threadIdx.x] = 0.0;
     if (threadIdx.x < EPIB_OUT_I) out_i[(size_t)pair * EPIB_OUT_I + threadIdx.x] = 0;
   }
-  if (h >= H || n < 8) return;
+  if (h >= H || n < 4) return;
   homo_hypothesis(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, seed, h, Hs + (size_t)pair * H * 9, valid + (size_t)pair * H);
 }
 
@@ -944,7 +897,7 @@ __global__ void __launch_bounds__(256)
 k_homo_score_batch(const float *__restrict__ p1, const float *__restrict__ p2, const int32_t *__restrict__ pn, int cap, HomoCam cam, double thr2,
                    int H, const double *__restrict__ Hs, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
   const int pair = blockIdx.y, n = pn[pair];
-  if (n < 8) return;
+  if (n < 4) return;
   const size_t oh = (size_t)pair * H;
   homo_score_run(p1 + (size_t)pair * cap * 2, p2 + (size_t)pair * cap * 2, n, cam, thr2, H, Hs + oh * 9, valid + oh, counts + oh, blockIdx.x, gridDim.x);
 }
@@ -955,7 +908,7 @@ k_homo_finish_batch(const float *__restrict__ p1, const float *__restrict__ p2, 
                     int H, const double *__restrict__ Hs, const int32_t *__restrict__ counts, double *__restrict__ out_d,
                     int32_t *__restrict__ out_i, int32_t *__restrict__ inl) {
   const int pair = blockIdx.x / cooperative_groups::this_cluster().num_blocks(), n = pn[pair];
-  if (n < 8) return;                                 // the whole cluster
+  if (n < 4) return;                                 // the whole cluster
   const size_t op = (size_t)pair * cap, oh = (size_t)pair * H;
   homo_finish_run(p1 + op * 2, p2 + op * 2, n, cam, thr2, H, Hs + oh * 9, counts + oh, out_d + (size_t)pair * EPIB_OUT_D,
                   out_i + (size_t)pair * EPIB_OUT_I, inl + op);

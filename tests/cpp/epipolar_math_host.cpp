@@ -16,8 +16,8 @@ int epi_decompose_homography(const double *H, double *Rs, double *ts, double *ns
 int epi_filter_homography(const double *Rs, const double *ns, int n_sol, const float *np1, const float *np2, const int *inl, int n_in, int *keep) {
   return epi::filter_homography_solutions(Rs, ns, n_sol, np1, np2, inl, n_in, keep);
 }
-// the local optimisation of k_homo_finish, serially: `rounds` times re-select the consensus set of the current H (scaled
-// coordinates, squared threshold thr2), then up to `iters` Gauss-Newton steps on it (csrc/epipolar.cu, k_homo_finish)
+// the local optimisation of k_homo_finish_batch, serially: `rounds` times re-select the consensus set of the current H (scaled
+// coordinates, squared threshold thr2), then up to `iters` Gauss-Newton steps on it (csrc/epipolar_kernels.cuh, homo_finish_run)
 int epi_homography_lo(const double *xy1, const double *xy2, int n, double thr2, int rounds, int iters, double *H) {
   int steps = 0;
   for (int round = 0; round < rounds; ++round) {

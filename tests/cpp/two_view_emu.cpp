@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE (CPU tier): the two-view kernels (csrc/epipolar_kernels.cuh — essential matrix, triangulation,
 // homography) built for the host with tests/cpp/cuda_emu.h and launched the way csrc/epipolar.cu launches them
-// (mvo_esti_motion_by_essential, mvo_esti_motion_by_homography, mvo_do_triangulation: same grids, same thresholds, same
-// post-processing).  The essential-matrix kernels have run on hardware; the homography kernels have not — this is their
+// (mvo_esti_motion_by_essential, mvo_esti_motion_by_homography, mvo_do_triangulation: the batch kernels with one pair and
+// cap = n, same thresholds, same post-processing).  The essential-matrix kernels have run on hardware; the homography kernels have not — this is their
 // first execution of any kind.
 #include "cuda_emu.h"
 
@@ -23,11 +23,13 @@ int emu_essential(const float *p1, const float *p2, int n, const double *K, doub
   const double thr2 = (threshold / cam.f) * (threshold / cam.f);
   std::vector<double> Es((size_t)H * 9), out(64, 0.0);
   std::vector<int32_t> valid((size_t)H), counts((size_t)H), oi(64, 0);
-  run_grid((unsigned)((H + 127) / 128), 1, 1, 128, 0, [&] { k_epi_hypotheses(p1, p2, n, cam, seed, H, Es.data(), valid.data()); });
+  const int32_t pn[1] = {n};
+  run_grid((unsigned)((H + 127) / 128), 1, 1, 128, 0, [&] { k_epi_hypotheses_batch(p1, p2, pn, n, cam, seed, H, Es.data(), valid.data()); });
   const int grid = std::min((H + 7) / 8, 64);                    // any grid covers all hypotheses (grid-stride loop)
-  run_grid((unsigned)grid, 1, 1, 256, (size_t)n * 32, [&] { k_epi_score(p1, p2, n, cam, thr2, H, Es.data(), valid.data(), counts.data()); });
-  run_clusters(EFIN_C, EFIN_C, EFIN_T, sizeof(EpiFinSmem), [&] { k_epi_finish(p1, p2, n, cam, thr2, H, Es.data(), counts.data(), out.data(), oi.data(), inliers); });
-  run_grid((unsigned)((n + 63) / 64), 1, 1, 256, 0, [&] { k_epi_vote(p1, p2, cam, out.data(), oi.data(), inliers); });
+  run_grid((unsigned)grid, 1, 1, 256, (size_t)n * 32, [&] { k_epi_score_batch(p1, p2, pn, n, cam, thr2, H, Es.data(), valid.data(), counts.data()); });
+  run_clusters(EFIN_C, EFIN_C, EFIN_T, sizeof(EpiFinSmem),
+               [&] { k_epi_finish_batch(p1, p2, pn, n, cam, thr2, H, Es.data(), counts.data(), out.data(), oi.data(), inliers); });
+  run_grid((unsigned)((n + 63) / 64), 1, 1, 256, 0, [&] { k_epi_vote_batch(p1, p2, pn, n, cam, out.data(), oi.data(), inliers); });
   // recoverPose's choice on the host, as mvo_esti_motion_by_essential does it: the first candidate whose vote count is a maximum
   const int32_t *g = oi.data() + 8;
   int pick = 3;
@@ -51,10 +53,13 @@ int emu_homography(const float *p1, const float *p2, int n, const double *K, dou
   const double thr2 = (threshold / cam.f) * (threshold / cam.f);
   std::vector<double> Hs((size_t)H * 9), out(64, 0.0);
   std::vector<int32_t> valid((size_t)H), counts((size_t)H), oi(64, 0);
-  run_grid((unsigned)((H + 127) / 128), 1, 1, 128, 0, [&] { k_homo_hypotheses(p1, p2, n, cam, seed, H, Hs.data(), valid.data()); });
+  const int32_t pn[1] = {n};
+  run_grid((unsigned)((H + 127) / 128), 1, 1, 128, 0,
+           [&] { k_homo_hypotheses_batch(p1, p2, pn, n, cam, seed, H, Hs.data(), valid.data(), out.data(), oi.data()); });
   const int grid = std::min((H + 7) / 8, 64);
-  run_grid((unsigned)grid, 1, 1, 256, (size_t)n * 32, [&] { k_homo_score(p1, p2, n, cam, thr2, H, Hs.data(), valid.data(), counts.data()); });
-  run_clusters(EFIN_C, EFIN_C, EFIN_T, sizeof(HomoFinSmem), [&] { k_homo_finish(p1, p2, n, cam, thr2, H, Hs.data(), counts.data(), out.data(), oi.data(), inliers); });
+  run_grid((unsigned)grid, 1, 1, 256, (size_t)n * 32, [&] { k_homo_score_batch(p1, p2, pn, n, cam, thr2, H, Hs.data(), valid.data(), counts.data()); });
+  run_clusters(EFIN_C, EFIN_C, EFIN_T, sizeof(HomoFinSmem),
+               [&] { k_homo_finish_batch(p1, p2, pn, n, cam, thr2, H, Hs.data(), counts.data(), out.data(), oi.data(), inliers); });
   if (getenv("MVO_EPI_DEBUG")) fprintf(stderr, "emu_homography: n %d inliers %d GN iterations %d\n", n, oi[0], oi[5]);
   memcpy(Hout, out.data(), 72);
   memcpy(out_i, oi.data(), 5 * sizeof(int32_t));

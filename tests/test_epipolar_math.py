@@ -157,7 +157,7 @@ def test_homography_from_4_and_transfer_error(epi):
 
 
 def test_homography_local_optimisation(epi):
-    """The Gauss-Newton refinement k_homo_finish applies to the best four-point model (same header functions, run serially):
+    """The Gauss-Newton refinement k_homo_finish_batch applies to the best four-point model (same header functions, run serially):
     from a minimal model fitted to NOISY points it reaches the least-squares homography of the consensus set — as good as
     cv2.findHomography's own refinement on the noise-free plane — and stops by itself."""
     cv2 = pytest.importorskip("cv2")

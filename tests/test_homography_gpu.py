@@ -101,6 +101,21 @@ for planar in (False, True):
         assert min(errs) < 0.03, errs                              # the true motion is among the surviving homography solutions
     sols_inv, _, _ = ctx.estimate_relative_poses(p1, p2, K, motion_cam2_to_cam1=False)
     assert np.allclose(sols_inv[0]["R"], sols[0]["R"].T, atol=1e-12) and np.allclose(sols_inv[0]["t"], -sols[0]["R"].T @ sols[0]["t"], atol=1e-12)
+# six correspondences of an exactly planar scene: fewer than the essential matrix needs, enough for a homography
+rng = np.random.default_rng(6)
+n = 6
+R, t = rod(np.array([0.02, -0.03, 0.01])), np.array([0.3, 0.02, 0.05])
+nrm = np.array([0.1, -0.05, 1.0]) / np.linalg.norm([0.1, -0.05, 1.0])
+P = np.stack([rng.uniform(-2, 2, n), rng.uniform(-1.5, 1.5, n), np.zeros(n)], 1)
+P[:, 2] = (4.0 - P[:, :2] @ nrm[:2]) / nrm[2]
+P2 = P @ R.T + t
+p1 = (P[:, :2] / P[:, 2:3] * K[0, 0] + K[:2, 2]).astype(np.float32)
+p2 = (P2[:, :2] / P2[:, 2:3] * K[0, 0] + K[:2, 2]).astype(np.float32)
+H, Rs, ts, ns, inl = ctx.esti_motion_by_homography(p1, p2, K, 3.0)          # raises unless the call returns MVO_OK
+assert len(inl) >= 4
+assert inl.tolist() == list(range(6)) and abs(H[2, 2] - 1) < 1e-12, (inl, H)
+m = np.c_[p1.astype(np.float64), np.ones(n)] @ H.T
+assert np.abs(m[:, :2] / m[:, 2:3] - p2).max() < 1e-3
 try:
     ctx.esti_motion_by_homography(np.zeros((3, 2), np.float32), np.zeros((3, 2), np.float32), K)
     raise SystemExit("n < 4 was accepted")

@@ -63,7 +63,7 @@ def _dir_err(a, b):
 
 
 @pytest.mark.parametrize("seed", [0, 1])
-def test_essential_kernels_on_the_cpu(emu, seed):
+def test_essential_kernels_as_a_batch_of_one(emu, seed):
     from oracle import epipolar_oracle
     p1, p2, R_true, t_true, good, X1 = _general_scene(seed)
     n = len(p1)
@@ -91,7 +91,7 @@ def test_essential_kernels_on_the_cpu(emu, seed):
 
 
 @pytest.mark.parametrize("seed", [0, 1, 2])
-def test_homography_kernels_on_the_cpu(emu, seed):
+def test_homography_kernels_as_a_batch_of_one(emu, seed):
     from oracle import epipolar_oracle
     rng = np.random.default_rng(seed)
     n = 320
@@ -128,3 +128,24 @@ def test_homography_kernels_on_the_cpu(emu, seed):
     inside = np.zeros(n, bool)
     inside[inl] = True
     assert (err[inside] <= 3.0 + 1e-6).all() and (err[~inside] > 3.0 - 1e-6).all()
+
+
+def test_homography_kernels_on_six_exact_points(emu):
+    """Six correspondences of an exactly planar scene: fewer than the essential matrix needs, enough for a homography, which
+    mvo_esti_motion_by_homography accepts from 4 correspondences on."""
+    rng = np.random.default_rng(6)
+    n = 6
+    R, t = _rod(np.array([0.02, -0.03, 0.01])), np.array([0.3, 0.02, 0.05])
+    nrm = np.array([0.1, -0.05, 1.0]) / np.linalg.norm([0.1, -0.05, 1.0])
+    P = np.stack([rng.uniform(-2, 2, n), rng.uniform(-1.5, 1.5, n), np.zeros(n)], 1)
+    P[:, 2] = (4.0 - P[:, :2] @ nrm[:2]) / nrm[2]
+    P2 = P @ R.T + t
+    p1 = (P[:, :2] / P[:, 2:3] * K[0, 0] + K[:2, 2]).astype(np.float32)
+    p2 = (P2[:, :2] / P2[:, 2:3] * K[0, 0] + K[:2, 2]).astype(np.float32)
+    H, inl, oi = np.zeros((3, 3)), np.zeros(n, np.int32), np.zeros(8, np.int32)
+    Kc = np.ascontiguousarray(K, np.float64)
+    ni = emu.emu_homography(p1.ctypes.data, p2.ctypes.data, n, Kc.ctypes.data, 3.0, HYP, 777, H.ctypes.data, inl.ctypes.data, oi.ctypes.data)
+    assert ni >= 4                                                  # mvo_esti_motion_by_homography returns MVO_OK
+    assert ni == 6 and inl.tolist() == list(range(6)) and abs(H[2, 2] - 1) < 1e-12
+    m = np.c_[p1.astype(np.float64), np.ones(n)] @ H.T
+    assert np.abs(m[:, :2] / m[:, 2:3] - p2).max() < 1e-3
