@@ -180,15 +180,15 @@ void mvo_destroy(mvo_ctx *ctx) {
   cudaStreamSynchronize(ctx->stream);
   orb_state_free(ctx);
   orb_tma_free(ctx);
-  DevBuf *dbs[] = {&ctx->d_a, &ctx->d_b, &ctx->d_c, &ctx->d_d, &ctx->d_e, &ctx->d_f, &ctx->orb_planes,
+  DevBuf *dbs[] = {&ctx->d_b, &ctx->d_c, &ctx->d_d, &ctx->d_f, &ctx->orb_planes,
                    &ctx->orb_cand, &ctx->orb_bandcnt, &ctx->orb_sel, &ctx->orb_misc, &ctx->orb_in,
                    &ctx->orb_kpts, &ctx->orb_desc, &ctx->orb_counts, &ctx->match_part,
                    &ctx->match_tickets, &ctx->match_in, &ctx->match_keys, &ctx->matchb_part, &ctx->matchb_tickets,
-                   &ctx->matchb_keys, &ctx->epib_buf, &ctx->pnp_pts, &ctx->pnp_hyp,
+                   &ctx->matchb_keys, &ctx->epib_buf, &ctx->epi_ess_buf, &ctx->epi_homo_buf, &ctx->pnp_pts, &ctx->pnp_hyp,
                    &ctx->pnp_cnt, &ctx->pnp_out, &ctx->ba_buf};
   for (DevBuf *b : dbs)
     if (b->p) cudaFree(b->p);
-  PinBuf *pbs[] = {&ctx->h_a, &ctx->h_b, &ctx->h_c, &ctx->orb_h, &ctx->match_h};
+  PinBuf *pbs[] = {&ctx->h_a, &ctx->h_b, &ctx->epi_ess_h, &ctx->epi_homo_h, &ctx->orb_h, &ctx->match_h};
   for (PinBuf *b : pbs)
     if (b->p) cudaFreeHost(b->p);
   for (const MvoEvPair &p : ctx->ev_pending) { cudaEventDestroy(p.a); cudaEventDestroy(p.b); }

@@ -16,8 +16,10 @@
 //   k_epi_vote_batch        recoverPose's cheirality vote, one thread per (inlier, candidate)
 //   k_triangulate           one thread per point: epi::triangulate_dlt
 // Every RANSAC kernel, essential and homography (k_homo_*_batch), has a pair dimension (one pair per blockIdx.y, one finish
-// cluster per pair).  The batch calls run them over the matched frame pairs of a batch, with recoverPose's pick on the device
-// (k_epi_pick); the single-pair calls run them as a batch of one (cap = n, pn[0] = n uploaded with the points) and pick on the host.
+// cluster per pair).  The batch calls run them over the matched frame pairs of a batch; the single-pair calls run them as a batch
+// of one (cap = n, pn[0] = n uploaded with the points), with the same row layout (ransac_rows).  What follows the RANSACs is
+// written once for host and device: recoverPose's pick (epi::recover_pose_pick, in k_epi_pick and mvo_epi_essential_end) and the
+// homography motions (epi::homography_motions, in mvo_epi_homography_end and two_view_batch.cu).
 // The numerics live in epipolar_math.cuh and are unit-tested on the host (tests/test_epipolar_math.py).
 #include <cooperative_groups.h>
 #include <stdlib.h>
@@ -81,16 +83,14 @@ __global__ void k_epi_math_test(const double *__restrict__ in, double *__restric
 // all block state in dynamic shared memory
 template <class K, class... A>
 cudaError_t launch_finish_cluster(mvo_ctx *ctx, unsigned clusters, size_t smem, K kernel, A... args) {
-  static const int env_c = getenv("MVO_EFIN_CLUSTER") ? atoi(getenv("MVO_EFIN_CLUSTER")) : EFIN_C;     // A/B hook: CTAs per cluster
-  const int csz = (env_c >= 1 && env_c <= 8) ? env_c : EFIN_C;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(csz * clusters);
+  cfg.gridDim = dim3(EFIN_C * clusters);
   cfg.blockDim = dim3(EFIN_T);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = csz;
+  attr[0].val.clusterDim.x = EFIN_C;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
@@ -151,14 +151,36 @@ int epi_batch_check(mvo_ctx *ctx, const char *what, int batch, int cap, int n_pa
   return MVO_OK;
 }
 
-// One RANSAC's device rows for n_pairs pairs (epipolar_kernels.cuh, "batch of frame pairs"): points and pn, hypothesis rows (72 B
-// model, valid, count), finish outputs and inlier lists.  A single-pair call lays them out for one pair with cap = n.
+// Blocks one after the other at 256-byte boundaries from base.  A layout runs twice: with base == nullptr it only measures (`end`),
+// then it runs again over the buffer reserved for that many bytes.
+struct Blocks {
+  uint8_t *base;
+  size_t end = 0;
+  template <class T> T *take(size_t count) {
+    T *p = base ? (T *)(base + end) : nullptr;
+    end = (end + count * sizeof(T) + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
+// One RANSAC's device rows for n_pairs pairs (epipolar_kernels.cuh, "batch of frame pairs"), inputs first and outputs last: points
+// and pn, hypothesis rows (72 B model, valid, count), finish outputs and inlier lists.  The batch calls and the single-pair jobs
+// (one pair, cap = n) both lay them out here.
 struct RansacRows {
   float *p1, *p2;
   int32_t *pn;
   double *models, *od;
   int32_t *valid, *cnt, *oi, *inl;
 };
+
+RansacRows ransac_rows(Blocks &L, int n_pairs, int cap, int H) {
+  const size_t np = (size_t)n_pairs, nh = np * H;
+  RansacRows r;
+  r.p1 = L.take<float>(np * cap * 2); r.p2 = L.take<float>(np * cap * 2); r.pn = L.take<int32_t>(np);
+  r.models = L.take<double>(nh * 9); r.valid = L.take<int32_t>(nh); r.cnt = L.take<int32_t>(nh);
+  r.od = L.take<double>(np * EPIB_OUT_D); r.oi = L.take<int32_t>(np * EPIB_OUT_I); r.inl = L.take<int32_t>(np * cap);
+  return r;
+}
 
 // The launch geometry of both RANSACs for n_pairs pairs of at most cap correspondences.  One focal length f = (fx + fy) / 2
 // (epipolar_geometry.cpp:26-27) and thr2 = (threshold / f)^2: findEssentialMat divides the threshold by the focal length, the
@@ -224,12 +246,11 @@ int epi_homography_enqueue(mvo_ctx *ctx, const RansacRows &r, int cap, int n_pai
   return MVO_OK;
 }
 
-// The scratch of both batch calls in ctx->epib_buf, for n_pairs pairs of at most cap correspondences: the gathered pixel points
-// (with tri also the normalised-plane points), pn, the hypothesis rows (80 B per hypothesis) and the essential finish outputs.  With
-// rel (mvo_estimate_relative_poses_batch_dev; tri must be set too) also the homography finish outputs, the internal essential
-// records, both inlier rows and the (R | t) of every solution.  The homography rows reuse the hypothesis rows, which
-// k_epi_finish_batch has consumed by the time k_homo_hypotheses_batch runs on the same stream.  e.inl is left to the caller
-// unless rel.
+// The scratch of both batch calls in ctx->epib_buf, for n_pairs pairs of at most cap correspondences: the essential RANSAC's rows
+// (with tri also the normalised-plane points).  With rel (mvo_estimate_relative_poses_batch_dev; tri must be set too) also the
+// homography finish outputs and inlier rows, the internal essential records and the (R | t) of every solution.  The homography rows
+// reuse the points and the hypothesis rows, which k_epi_finish_batch has consumed by the time k_homo_hypotheses_batch runs on the
+// same stream.  Without rel the caller points e.inl at its own inlier rows.
 struct EpiBatchScratch {
   RansacRows e, h;
   float *np1, *np2;
@@ -238,31 +259,56 @@ struct EpiBatchScratch {
 };
 
 int epi_batch_scratch(mvo_ctx *ctx, int n_pairs, int cap, bool tri, bool rel, EpiBatchScratch *b) {
-  const size_t np = (size_t)n_pairs, H = (size_t)ctx->prm.epi_hypotheses, pts = np * cap * 8, idx = np * cap * 4;
-  size_t end = 0;
-  auto take = [&end](size_t bytes) { const size_t at = end; end = (end + bytes + 255) & ~(size_t)255; return at; };
-  const size_t o_p1 = take(pts), o_p2 = take(pts), o_n1 = tri ? take(pts) : 0, o_n2 = tri ? take(pts) : 0, o_pn = take(np * 4);
-  const size_t o_E = take(np * H * 72), o_valid = take(np * H * 4), o_cnt = take(np * H * 4);
-  const size_t o_od = take(np * EPIB_OUT_D * 8), o_oi = take(np * EPIB_OUT_I * 4);
-  size_t o_hd = 0, o_hi = 0, o_ess = 0, o_ie = 0, o_ih = 0, o_rt = 0;
-  if (rel) {
-    o_hd = take(np * EPIB_OUT_D * 8); o_hi = take(np * EPIB_OUT_I * 4); o_ess = take(np * sizeof(mvo_two_view_result));
-    o_ie = take(idx); o_ih = take(idx); o_rt = take(np * 5 * 12 * 8);
-  }
-  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, end));
-  uint8_t *d = (uint8_t *)ctx->epib_buf.p;
-  *b = EpiBatchScratch();
-  RansacRows &e = b->e;
-  e.p1 = (float *)(d + o_p1); e.p2 = (float *)(d + o_p2); e.pn = (int32_t *)(d + o_pn);
-  e.models = (double *)(d + o_E); e.valid = (int32_t *)(d + o_valid); e.cnt = (int32_t *)(d + o_cnt);
-  e.od = (double *)(d + o_od); e.oi = (int32_t *)(d + o_oi);
-  if (tri) { b->np1 = (float *)(d + o_n1); b->np2 = (float *)(d + o_n2); }
-  if (rel) {
-    e.inl = (int32_t *)(d + o_ie);
-    b->h = e;
-    b->h.od = (double *)(d + o_hd); b->h.oi = (int32_t *)(d + o_hi); b->h.inl = (int32_t *)(d + o_ih);
-    b->ess = (mvo_two_view_result *)(d + o_ess); b->rt = (double *)(d + o_rt);
-  }
+  const size_t np = (size_t)n_pairs, pts = np * cap * 2;
+  auto lay = [&](uint8_t *base) {
+    Blocks L{base};
+    *b = EpiBatchScratch();
+    b->e = ransac_rows(L, n_pairs, cap, ctx->prm.epi_hypotheses);
+    if (tri) { b->np1 = L.take<float>(pts); b->np2 = L.take<float>(pts); }
+    if (rel) {
+      b->h = b->e;
+      b->h.od = L.take<double>(np * EPIB_OUT_D); b->h.oi = L.take<int32_t>(np * EPIB_OUT_I); b->h.inl = L.take<int32_t>(np * cap);
+      b->ess = L.take<mvo_two_view_result>(np); b->rt = L.take<double>(np * 5 * 12);
+    }
+    return L.end;
+  };
+  MVO_TRY(mvo_reserve(ctx, ctx->epib_buf, lay(nullptr)));
+  lay((uint8_t *)ctx->epib_buf.p);
+  return MVO_OK;
+}
+
+// The single-pair job of either RANSAC, a batch of one (cap = n) in the job's own buffers: pts1 / pts2 / pn staged and uploaded in
+// one copy, the model's RANSAC (essential with recoverPose's vote when vote, else homography), the finish outputs and the inlier
+// list queued back in one copy; nothing waits.  `extra` more bytes of both buffers are the caller's (*d_extra, *h_extra).
+int epi_job_begin(mvo_ctx *ctx, DevBuf &dbuf, PinBuf &hbuf, bool essential, const float *pts1, const float *pts2, int n, const double *K,
+                  double threshold, bool vote, size_t extra, uint8_t **d_extra, uint8_t **h_extra, MvoEpiJob *job) {
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int H = ctx->prm.epi_hypotheses;
+  Blocks L{nullptr};
+  ransac_rows(L, 1, n, H);
+  MVO_TRY(mvo_reserve(ctx, dbuf, L.end + extra));
+  uint8_t *d = (uint8_t *)dbuf.p;
+  L = Blocks{d};
+  const RansacRows r = ransac_rows(L, 1, n, H);
+  // pinned staging: the inputs at their device offsets, then the outputs from od to the end of the inlier list, then the extra
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  uint8_t *od = (uint8_t *)r.od;
+  const size_t in = (uint8_t *)(r.pn + 1) - d, o_res = al(in), res = (uint8_t *)(r.inl + n) - od, o_extra = al(o_res + res);
+  MVO_TRY(mvo_reserve_pinned(ctx, hbuf, o_extra + extra));
+  uint8_t *h = (uint8_t *)hbuf.p, *hr = h + o_res;
+  memcpy(h + ((uint8_t *)r.p1 - d), pts1, (size_t)n * 8);
+  memcpy(h + ((uint8_t *)r.p2 - d), pts2, (size_t)n * 8);
+  memcpy(h + ((uint8_t *)r.pn - d), &n, 4);
+  MVO_CUDA(ctx, cudaMemcpyAsync(d, h, in, cudaMemcpyHostToDevice, ctx->stream));
+  RansacGeom g;
+  if (essential) MVO_TRY(epi_essential_enqueue(ctx, r, n, 1, K, threshold, vote, &g));
+  else MVO_TRY(epi_homography_enqueue(ctx, r, n, 1, K, threshold, &g));
+  MVO_CUDA(ctx, cudaMemcpyAsync(hr, od, res, cudaMemcpyDeviceToHost, ctx->stream));
+  memset(job, 0, sizeof *job);
+  job->stream = ctx->stream; job->n = n; job->H = H; job->thr2 = g.thr2; job->f = g.f;
+  job->h_out = (double *)hr; job->h_oi = (int32_t *)(hr + ((uint8_t *)r.oi - od)); job->h_inl = (int32_t *)(hr + ((uint8_t *)r.inl - od));
+  job->d_valid = r.valid; job->d_cnt = r.cnt; job->d_model = r.models;
+  if (d_extra) { *d_extra = d + L.end; *h_extra = h + o_extra; }
   return MVO_OK;
 }
 
@@ -369,64 +415,34 @@ int mvo_epi_essential_begin(mvo_ctx *ctx, const float *pts1, const float *pts2, 
   if (!((K[0] + K[4]) / 2 > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal length must be positive");
   if ((size_t)n * 4 * sizeof(double) > 200 * 1024)
     return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByEssential: more than %d correspondences", 200 * 1024 / 32);
-  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int H = ctx->prm.epi_hypotheses;
-  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  // a batch of one: pn[0] = n follows p2 in the same copy
-  const size_t o_p1 = 0, o_p2 = al(o_p1 + (size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8 + 4), o_E = al(o_inl + (size_t)n * 4);
-  const size_t o_valid = al(o_E + (size_t)H * 72), o_cnt = al(o_valid + (size_t)H * 4), o_out = al(o_cnt + (size_t)H * 4);
-  // optional triangulation block: np1, np2 (n x 2 floats each), R | t (12 doubles), out (n x 3 floats)
-  const size_t o_t1 = al(o_out + 512), o_t2 = al(o_t1 + (size_t)n * 8), o_trt = al(o_t2 + (size_t)n * 8), o_tout = al(o_trt + 96);
-  const size_t o_end = tri ? o_tout + (size_t)n * 12 : o_out + 512;
-  // pinned staging: [p1 p2 pn | np1 np2 Rt] in, [out block 512 B + inliers | triangulated points] out
-  const size_t h_in = al((size_t)n * 16 + 4) + (tri ? al((size_t)n * 16) + 256 : 0), h_res = 512 + al((size_t)n * 4) + 256;
-  MVO_TRY(mvo_reserve(ctx, ctx->d_a, o_end));
-  MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_a, h_in + h_res + (tri ? (size_t)n * 12 : 0) + 1024));
-  uint8_t *d = (uint8_t *)ctx->d_a.p, *h = (uint8_t *)ctx->h_a.p;
-  memcpy(h, pts1, (size_t)n * 8);
-  memcpy(h + (size_t)n * 8, pts2, (size_t)n * 8);
-  memcpy(h + (size_t)n * 16, &n, 4);
-  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p1, h, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p2, h + (size_t)n * 8, (size_t)n * 8 + 4, cudaMemcpyHostToDevice, ctx->stream));
+  // the triangulation block after the RANSAC's, laid out alike in both buffers: np1, np2 (n x 2 floats each), R | t (12 doubles) in,
+  // n x 3 floats out
+  const size_t tri_in = (size_t)n * 16 + 96, o_tout = (tri_in + 255) & ~(size_t)255;
+  uint8_t *d, *h;
+  MVO_TRY(epi_job_begin(ctx, ctx->epi_ess_buf, ctx->epi_ess_h, true, pts1, pts2, n, K, threshold, want_pose != 0, tri ? o_tout + (size_t)n * 12 : 0,
+                        &d, &h, job));
+  job->want_pose = want_pose != 0; job->tri = tri; job->tri_stream = ctx->stream;
+  if (!tri) return MVO_OK;
   // the triangulation does not depend on the RANSAC: it runs on the context's side stream next to it (on the same stream when
   // per-kernel event timing is on, or when this job itself was pointed at the side stream)
-  cudaStream_t tri_stream = ctx->stream;
-  float *h_tri = (float *)(h + h_in + h_res);
-  if (tri) {
-    cudaStream_t side = ctx->timing_mask ? nullptr : mvo_side_stream(ctx);
-    if (side && side != ctx->stream) tri_stream = side;
-    uint8_t *ht = h + al((size_t)n * 16 + 4);
-    memcpy(ht, tri_np1, (size_t)n * 8);
-    memcpy(ht + (size_t)n * 8, tri_np2, (size_t)n * 8);
-    memcpy(ht + al((size_t)n * 16), tri_R, 72);
-    memcpy(ht + al((size_t)n * 16) + 72, tri_t, 24);
-    MVO_CUDA(ctx, cudaMemcpyAsync(d + o_t1, ht, (size_t)n * 8, cudaMemcpyHostToDevice, tri_stream));
-    MVO_CUDA(ctx, cudaMemcpyAsync(d + o_t2, ht + (size_t)n * 8, (size_t)n * 8, cudaMemcpyHostToDevice, tri_stream));
-    MVO_CUDA(ctx, cudaMemcpyAsync(d + o_trt, ht + al((size_t)n * 16), 96, cudaMemcpyHostToDevice, tri_stream));
-    {
-      cudaStream_t keep = ctx->stream;
-      ctx->stream = tri_stream;              // KTimer records on ctx->stream
-      { KTimer kt(ctx, KC_EPI);
-      k_triangulate<<<(n + 127) / 128, 128, 0, tri_stream>>>((const float *)(d + o_t1), (const float *)(d + o_t2), nullptr, n, (const double *)(d + o_trt),
-                                                              (float *)(d + o_tout)); }
-      ctx->stream = keep;
-    }
-    MVO_CHECK_LAUNCH(ctx);
-    MVO_CUDA(ctx, cudaMemcpyAsync(h_tri, d + o_tout, (size_t)n * 12, cudaMemcpyDeviceToHost, tri_stream));
+  cudaStream_t tri_stream = ctx->stream, side = ctx->timing_mask ? nullptr : mvo_side_stream(ctx);
+  if (side && side != ctx->stream) tri_stream = side;
+  memcpy(h, tri_np1, (size_t)n * 8);
+  memcpy(h + (size_t)n * 8, tri_np2, (size_t)n * 8);
+  memcpy(h + (size_t)n * 16, tri_R, 72);
+  memcpy(h + (size_t)n * 16 + 72, tri_t, 24);
+  MVO_CUDA(ctx, cudaMemcpyAsync(d, h, tri_in, cudaMemcpyHostToDevice, tri_stream));
+  {
+    cudaStream_t keep = ctx->stream;
+    ctx->stream = tri_stream;              // KTimer records on ctx->stream
+    { KTimer kt(ctx, KC_EPI);
+    k_triangulate<<<(n + 127) / 128, 128, 0, tri_stream>>>((const float *)d, (const float *)(d + (size_t)n * 8), nullptr, n,
+                                                            (const double *)(d + (size_t)n * 16), (float *)(d + o_tout)); }
+    ctx->stream = keep;
   }
-  RansacRows r;
-  r.p1 = (float *)(d + o_p1); r.p2 = (float *)(d + o_p2); r.pn = (int32_t *)(d + o_p2 + (size_t)n * 8);
-  r.models = (double *)(d + o_E); r.valid = (int32_t *)(d + o_valid); r.cnt = (int32_t *)(d + o_cnt);
-  r.od = (double *)(d + o_out); r.oi = (int32_t *)(d + o_out + 256); r.inl = (int32_t *)(d + o_inl);
-  RansacGeom g;
-  MVO_TRY(epi_essential_enqueue(ctx, r, n, 1, K, threshold, want_pose != 0, &g));
-  double *h_out = (double *)(h + h_in);
-  int32_t *h_inl = (int32_t *)((uint8_t *)h_out + 512);
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_out, r.od, 512, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_inl, r.inl, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  job->tri_stream = tri_stream;
-  job->stream = ctx->stream; job->n = n; job->H = H; job->want_pose = want_pose != 0; job->tri = tri; job->thr2 = g.thr2; job->f = g.f;
-  job->h_out = h_out; job->h_inl = h_inl; job->h_tri = h_tri; job->d_valid = r.valid; job->d_cnt = r.cnt; job->d_model = r.models;
+  MVO_CHECK_LAUNCH(ctx);
+  MVO_CUDA(ctx, cudaMemcpyAsync(h + o_tout, d + o_tout, (size_t)n * 12, cudaMemcpyDeviceToHost, tri_stream));
+  job->tri_stream = tri_stream; job->h_tri = (float *)(h + o_tout);
   return MVO_OK;
 }
 
@@ -435,8 +451,8 @@ int mvo_epi_essential_end(mvo_ctx *ctx, MvoEpiJob *job, double *E, double *R, do
   MVO_CUDA(ctx, cudaStreamSynchronize(job->stream));
   if (job->tri && job->tri_stream != job->stream) MVO_CUDA(ctx, cudaStreamSynchronize(job->tri_stream));
   const int n = job->n, H = job->H;
-  double *h_out = job->h_out;
-  int32_t *h_i = (int32_t *)((uint8_t *)h_out + 256), *h_inl = job->h_inl;
+  const double *h_out = job->h_out;
+  const int32_t *h_i = job->h_oi, *h_inl = job->h_inl;
   if (job->tri && tri_out) memcpy(tri_out, job->h_tri, (size_t)n * 12);
   const int ni = h_i[0];
   if (getenv("MVO_EPI_DEBUG")) {
@@ -463,18 +479,7 @@ int mvo_epi_essential_end(mvo_ctx *ctx, MvoEpiJob *job, double *E, double *R, do
     *n_inliers = ni;
     return MVO_OK;
   }
-  // recoverPose's choice among (R1,t) (R2,t) (R1,-t) (R2,-t), OpenCV's order: the first candidate whose vote count is a maximum
-  const int32_t *g = h_i + 8;
-  int pick = 3;
-  if (g[0] >= g[1] && g[0] >= g[2] && g[0] >= g[3]) pick = 0;
-  else if (g[1] >= g[0] && g[1] >= g[2] && g[1] >= g[3]) pick = 1;
-  else if (g[2] >= g[0] && g[2] >= g[1] && g[2] >= g[3]) pick = 2;
-  h_i[2] = g[pick];
-  const double *tt = h_out + 27, sg = pick < 2 ? 1.0 : -1.0;
-  const double nt = sqrt(tt[0] * tt[0] + tt[1] * tt[1] + tt[2] * tt[2]);                 // t /= |t| (epipolar_geometry.cpp:54-55)
-  memcpy(E, h_out, 72);
-  memcpy(R, h_out + ((pick & 1) ? 18 : 9), 72);
-  for (int q = 0; q < 3; ++q) t[q] = sg * tt[q] / nt;
+  epi::recover_pose_pick(h_out, h_i + 8, E, R, t);
   memcpy(inliers, h_inl, (size_t)ni * 4);
   *n_inliers = ni;
   return MVO_OK;
@@ -496,7 +501,7 @@ int mvo_esti_motion_by_homography(mvo_ctx *ctx, const float *pts1, const float *
 
 }  // extern "C"
 
-// first half (own device / pinned scratch, so that it can run next to an essential-matrix job on another stream)
+// first half (own device / pinned buffers, so that it can run next to an essential-matrix job on another stream)
 int mvo_epi_homography_begin(mvo_ctx *ctx, const float *pts1, const float *pts2, int n, const double *K, double threshold, MvoEpiJob *job) {
   if (!ctx) return MVO_ERR_INVALID_ARG;
   if (!pts1 || !pts2 || !K || !job) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "estiMotionByHomography: null pointer");
@@ -505,40 +510,14 @@ int mvo_epi_homography_begin(mvo_ctx *ctx, const float *pts1, const float *pts2,
   if (!(K[0] > 0 && K[4] > 0)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "K: focal lengths must be positive");
   if ((size_t)n * 4 * sizeof(double) > 200 * 1024)
     return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "estiMotionByHomography: more than %d correspondences", 200 * 1024 / 32);
-  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int H = ctx->prm.epi_hypotheses;
-  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  // a batch of one: pn[0] = n follows p2 in the same copy
-  const size_t o_p1 = 0, o_p2 = al(o_p1 + (size_t)n * 8), o_inl = al(o_p2 + (size_t)n * 8 + 4), o_H = al(o_inl + (size_t)n * 4);
-  const size_t o_valid = al(o_H + (size_t)H * 72), o_cnt = al(o_valid + (size_t)H * 4), o_out = al(o_cnt + (size_t)H * 4), o_end = o_out + 512;
-  MVO_TRY(mvo_reserve(ctx, ctx->d_e, o_end));
-  MVO_TRY(mvo_reserve_pinned(ctx, ctx->h_c, al((size_t)n * 16 + 4) + (size_t)n * 4 + 1024));
-  uint8_t *d = (uint8_t *)ctx->d_e.p, *h = (uint8_t *)ctx->h_c.p;
-  memcpy(h, pts1, (size_t)n * 8);
-  memcpy(h + (size_t)n * 8, pts2, (size_t)n * 8);
-  memcpy(h + (size_t)n * 16, &n, 4);
-  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p1, h, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(d + o_p2, h + (size_t)n * 8, (size_t)n * 8 + 4, cudaMemcpyHostToDevice, ctx->stream));
-  RansacRows r;
-  r.p1 = (float *)(d + o_p1); r.p2 = (float *)(d + o_p2); r.pn = (int32_t *)(d + o_p2 + (size_t)n * 8);
-  r.models = (double *)(d + o_H); r.valid = (int32_t *)(d + o_valid); r.cnt = (int32_t *)(d + o_cnt);
-  r.od = (double *)(d + o_out); r.oi = (int32_t *)(d + o_out + 256); r.inl = (int32_t *)(d + o_inl);
-  RansacGeom g;
-  MVO_TRY(epi_homography_enqueue(ctx, r, n, 1, K, threshold, &g));
-  double *h_out = (double *)(h + al((size_t)n * 16 + 4));
-  int32_t *h_inl = (int32_t *)((uint8_t *)h_out + 512);
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_out, r.od, 512, cudaMemcpyDeviceToHost, ctx->stream));
-  MVO_CUDA(ctx, cudaMemcpyAsync(h_inl, r.inl, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  memset(job, 0, sizeof *job);
-  job->stream = ctx->stream; job->n = n; job->H = H; job->thr2 = g.thr2; job->f = g.f; job->h_out = h_out; job->h_inl = h_inl;
-  return MVO_OK;
+  return epi_job_begin(ctx, ctx->epi_homo_buf, ctx->epi_homo_h, false, pts1, pts2, n, K, threshold, false, 0, nullptr, nullptr, job);
 }
 
 int mvo_epi_homography_end(mvo_ctx *ctx, MvoEpiJob *job, const double *K, double *Hout, double *Rs, double *ts, double *normals, int *n_solutions,
                            int32_t *inliers, int *n_inliers) {
   MVO_CUDA(ctx, cudaStreamSynchronize(job->stream));
-  double *h_out = job->h_out;
-  int32_t *h_i = (int32_t *)((uint8_t *)h_out + 256), *h_inl = job->h_inl;
+  const double *h_out = job->h_out;
+  const int32_t *h_i = job->h_oi, *h_inl = job->h_inl;
   *n_solutions = 0;
   const int ni = h_i[0];
   if (ni < 4) {
@@ -550,18 +529,7 @@ int mvo_epi_homography_end(mvo_ctx *ctx, MvoEpiJob *job, const double *K, double
   memcpy(Hout, h_out, 72);
   memcpy(inliers, h_inl, (size_t)ni * 4);
   *n_inliers = ni;
-  // cv::decomposeHomographyMat(H, K) (:119-120) on the host: Hn = K^-1 H K, then t /= |t| (:122-126)
-  const double fx = K[0], fy = K[4], cx = K[2], cy = K[5];
-  const double Km[9] = {fx, 0, cx, 0, fy, cy, 0, 0, 1}, Ki[9] = {1 / fx, 0, -cx / fx, 0, 1 / fy, -cy / fy, 0, 0, 1};
-  double T[9], Hn[9];
-  epi::mat3_mul(Hout, Km, T);
-  epi::mat3_mul(Ki, T, Hn);
-  const int ns = epi::decompose_homography(Hn, Rs, ts, normals);
-  for (int s = 0; s < ns; ++s) {
-    const double nt = sqrt(ts[3 * s] * ts[3 * s] + ts[3 * s + 1] * ts[3 * s + 1] + ts[3 * s + 2] * ts[3 * s + 2]);
-    if (nt > 0) for (int q = 0; q < 3; ++q) ts[3 * s + q] /= nt;      // a pure rotation keeps t = 0 (the reference divides by zero here)
-  }
-  *n_solutions = ns;
+  *n_solutions = epi::homography_motions(Hout, K, Rs, ts, normals);
   return MVO_OK;
 }
 

@@ -395,7 +395,7 @@ __device__ __forceinline__ void epi_finish_run(const float *__restrict__ p1, con
     if (r < rank) off += c;
     n_in += c;
   }
-  // the consensus set, ascending; the cheirality vote of recoverPose runs in k_epi_vote_batch (all SMs), the pick on the host or in k_epi_pick
+  // the consensus set, ascending; the cheirality vote of recoverPose runs in k_epi_vote_batch (all SMs), the pick in epi::recover_pose_pick
   for (int i = b0; i < e0; ++i) {
     const double x1 = ((double)p1[2 * i] - cam.cx) / cam.f, y1 = ((double)p1[2 * i + 1] - cam.cy) / cam.f;
     const double x2 = ((double)p2[2 * i] - cam.cx) / cam.f, y2 = ((double)p2[2 * i + 1] - cam.cy) / cam.f;
@@ -542,9 +542,8 @@ k_epi_vote_batch(const float *__restrict__ p1, const float *__restrict__ p2, con
   epi_vote_run(p1 + op * 2, p2 + op * 2, cam, out_d + (size_t)pair * EPIB_OUT_D, out_i + (size_t)pair * EPIB_OUT_I, inl + op, blockIdx.x);
 }
 
-// recoverPose's choice among (R1,t) (R2,t) (R1,-t) (R2,-t) and t /= |t|, as mvo_epi_essential_end does on the host: the first
-// candidate whose vote count is a maximum.  |t| without contraction (the host's sum of three products), so t keeps the host's bits.
-// One thread per pair; a failed pair gets its status and nothing else.
+// recoverPose's pick (epi::recover_pose_pick, which mvo_epi_essential_end runs on the host) of every pair: one thread per pair; a
+// failed pair gets its status and nothing else.
 __global__ void __launch_bounds__(128)
 k_epi_pick(const int32_t *__restrict__ pn, int n_pairs, const double *__restrict__ out_d, const int32_t *__restrict__ out_i,
            mvo_two_view_result *__restrict__ res) {
@@ -555,18 +554,8 @@ k_epi_pick(const int32_t *__restrict__ pn, int n_pairs, const double *__restrict
   if (n < 0) { r.status = n; return; }
   const int32_t *oi = out_i + (size_t)pair * EPIB_OUT_I;
   if (n < 8 || oi[0] < 8) { r.status = MVO_ERR_DEGENERATE; return; }
-  const double *od = out_d + (size_t)pair * EPIB_OUT_D;
-  const int32_t *g = oi + 8;
-  int pick = 3;
-  if (g[0] >= g[1] && g[0] >= g[2] && g[0] >= g[3]) pick = 0;
-  else if (g[1] >= g[0] && g[1] >= g[2] && g[1] >= g[3]) pick = 1;
-  else if (g[2] >= g[0] && g[2] >= g[1] && g[2] >= g[3]) pick = 2;
-  const double *tt = od + 27, sg = pick < 2 ? 1.0 : -1.0;
-  const double nt = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(tt[0], tt[0]), __dmul_rn(tt[1], tt[1])), __dmul_rn(tt[2], tt[2])));
-  const double *Rp = od + ((pick & 1) ? 18 : 9);
-  for (int q = 0; q < 9; ++q) { r.E[q] = od[q]; r.R[q] = Rp[q]; }
-  for (int q = 0; q < 3; ++q) r.t[q] = __dmul_rn(sg, tt[q]) / nt;
-  r.status = MVO_OK; r.n_matches = n; r.n_inliers = oi[0]; r.votes = g[pick];
+  r.votes = epi::recover_pose_pick(out_d + (size_t)pair * EPIB_OUT_D, oi + 8, r.E, r.R, r.t);
+  r.status = MVO_OK; r.n_matches = n; r.n_inliers = oi[0];
 }
 
 // doTriangulation of every pair's inliers with that pair's (R, t)

@@ -8,9 +8,12 @@
 //   sampson_err              the squared Sampson distance OpenCV's findEssentialMat scores with (five-point.cpp)
 //   decompose_essential      R1, R2, t of cv::decomposeEssentialMat
 //   triangulate_dlt          one point of cv::triangulatePoints (the 4x4 homogeneous DLT, triangulate.cpp)
+//   recover_pose_pick        recoverPose's choice among the four (R, t) of an essential matrix, t /= |t|
+//   homography_motions       cv::decomposeHomographyMat(H, K), t /= |t|
 // fp64 throughout, no dynamic memory, fixed loop bounds.
 #pragma once
 #include <math.h>
+#include <stdint.h>
 
 #if defined(__CUDACC__)
 #define EPI_HD __host__ __device__ __forceinline__
@@ -351,6 +354,45 @@ EPI_HD_CALL int decompose_homography(const double *Hin, double *Rs, double *ts, 
     }
   }
   return 4;
+}
+
+// cv::decomposeHomographyMat(H, K) and t /= |t| (epipolar_geometry.cpp:119-126): Hn = K^-1 H K with K^-1 written out, then every
+// solution's t scaled to unit length; a pure rotation keeps t = 0 (the reference divides by zero there).  Returns the number of
+// solutions.  Both callers compile it without contraction (the host's g++ for x86-64, two_view_batch.cu with --fmad=false), so they
+// get the same bits.
+EPI_HD int homography_motions(const double *H, const double *K, double *Rs, double *ts, double *ns) {
+  const double fx = K[0], fy = K[4], cx = K[2], cy = K[5];
+  const double Km[9] = {fx, 0, cx, 0, fy, cy, 0, 0, 1}, Ki[9] = {1 / fx, 0, -cx / fx, 0, 1 / fy, -cy / fy, 0, 0, 1};
+  double T[9], Hn[9];
+  mat3_mul(H, Km, T);
+  mat3_mul(Ki, T, Hn);
+  const int n_sol = decompose_homography(Hn, Rs, ts, ns);
+  for (int s = 0; s < n_sol; ++s) {
+    double *t = ts + 3 * s;
+    const double nt = sqrt(t[0] * t[0] + t[1] * t[1] + t[2] * t[2]);
+    if (nt > 0) for (int q = 0; q < 3; ++q) t[q] /= nt;
+  }
+  return n_sol;
+}
+
+// recoverPose's choice among (R1,t) (R2,t) (R1,-t) (R2,-t) of an essential-matrix finish output block od (E at 0, R1 at 9, R2 at 18,
+// t at 27) with the four vote counts g: the first candidate whose count is a maximum (OpenCV's tie order), then t /= |t|
+// (epipolar_geometry.cpp:54-55).  Writes E, R, t and returns the pick's vote count.  |t| rounds each product and sum on its own on
+// both sides, so the device returns the host's bits; only its spelling differs.
+EPI_HD int recover_pose_pick(const double *od, const int32_t *g, double *E, double *R, double *t) {
+  int pick = 3;
+  if (g[0] >= g[1] && g[0] >= g[2] && g[0] >= g[3]) pick = 0;
+  else if (g[1] >= g[0] && g[1] >= g[2] && g[1] >= g[3]) pick = 1;
+  else if (g[2] >= g[0] && g[2] >= g[1] && g[2] >= g[3]) pick = 2;
+  const double *tt = od + 27, *Rp = od + ((pick & 1) ? 18 : 9), sg = pick < 2 ? 1.0 : -1.0;
+#ifdef __CUDA_ARCH__
+  const double nt = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(tt[0], tt[0]), __dmul_rn(tt[1], tt[1])), __dmul_rn(tt[2], tt[2])));
+#else
+  const double nt = sqrt(tt[0] * tt[0] + tt[1] * tt[1] + tt[2] * tt[2]);
+#endif
+  for (int q = 0; q < 9; ++q) { E[q] = od[q]; R[q] = Rp[q]; }
+  for (int q = 0; q < 3; ++q) t[q] = sg * tt[q] / nt;
+  return g[pick];
 }
 
 // cv::filterHomographyDecompByVisibleRefpoints (removeWrongRtOfHomography, epipolar_geometry.cpp:59-88): a solution

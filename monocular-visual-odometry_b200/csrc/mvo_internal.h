@@ -83,8 +83,8 @@ struct mvo_ctx {
   int sm_count = 0;
 
   // generic scratch
-  DevBuf d_a, d_b, d_c, d_d, d_e, d_f;
-  PinBuf h_a, h_b, h_c;
+  DevBuf d_b, d_c, d_d, d_f;
+  PinBuf h_a, h_b;
   cudaStream_t side_stream = nullptr;   // mvo_side_stream()
 
   // ORB workspace (sized for `orb_batch` frames of the current layout)
@@ -102,9 +102,12 @@ struct mvo_ctx {
   // batched matchFeatures (mvo_match_features_batch_dev): partial winners, merge tickets, packed keys of every pair
   DevBuf matchb_part, matchb_tickets, matchb_keys;
   // batched two-view calls (mvo_esti_motion_by_essential_batch_dev, mvo_estimate_relative_poses_batch_dev): points, hypotheses,
-  // counts and finish outputs of every pair; its own block, so that it never aliases the single-pair jobs' d_a / d_e that may run
-  // on the side stream
+  // counts and finish outputs of every pair; its own block, so that it never aliases the single-pair jobs' buffers
   DevBuf epib_buf;
+  // the single-pair essential-matrix and homography jobs (MvoEpiJob): device rows and pinned staging of each, so that the two can
+  // run side by side on two streams
+  DevBuf epi_ess_buf, epi_homo_buf;
+  PinBuf epi_ess_h, epi_homo_h;
 
   // timing
   uint32_t timing_mask = 0;
@@ -156,6 +159,13 @@ static inline MVO_HD void inv_rigid(const double *T, double *Ti) {        // [R 
   for (int i = 0; i < 3; ++i) r[i * 4 + 3] = -(r[i * 4] * T[3] + r[i * 4 + 1] * T[7] + r[i * 4 + 2] * T[11]);
   r[12] = r[13] = r[14] = 0; r[15] = 1;
   memcpy(Ti, r, sizeof r);
+}
+static inline MVO_HD void inv_rt(double *R, double *t) {                 // basics::invRt on a row-major R and t: R^T, -R^T t in place
+  double Rt[9], tt[3];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rt[i * 3 + j] = R[j * 3 + i];
+  for (int i = 0; i < 3; ++i) tt[i] = -(Rt[i * 3] * t[0] + Rt[i * 3 + 1] * t[1] + Rt[i * 3 + 2] * t[2]);
+  for (int q = 0; q < 9; ++q) R[q] = Rt[q];
+  for (int q = 0; q < 3; ++q) t[q] = tt[q];
 }
 static inline MVO_HD void rt_to_T(const double *R, const double *t, double *T) {      // basics::convertRt2T
   for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) T[i * 4 + j] = R[i * 3 + j]; T[i * 4 + 3] = t[i]; }
@@ -332,11 +342,12 @@ int mvo_match_filter_keys(mvo_ctx *ctx, int method_index, const uint32_t *keys, 
 // estiMotionByEssential with the keyframe branch's options: no recoverPose vote, triangulation of all correspondences in the same
 // submission (epipolar.cu)
 // the same, and estiMotionByHomography, split at the synchronisation: _begin enqueues everything on ctx->stream (which the caller may
-// point at ctx's side stream for the duration of the call), _end waits for that stream and post-processes.  The two estimations use
-// separate scratch buffers, so the initialisation runs them side by side (two_view.cpp).
+// point at ctx's side stream for the duration of the call), _end waits for that stream and post-processes.  Both jobs are a batch of
+// one laid out like the batch calls' rows (epipolar.cu), each in its own buffers (epi_ess_* and epi_homo_*), so the initialisation
+// runs them side by side (two_view.cpp).  h_out / h_oi: the finish outputs (EPIB_OUT_D doubles, EPIB_OUT_I ints) copied back.
 struct MvoEpiJob {
   cudaStream_t stream; int n, H; bool want_pose, tri; double thr2, f;
-  double *h_out; int32_t *h_inl; float *h_tri;
+  double *h_out; int32_t *h_oi, *h_inl; float *h_tri;
   cudaStream_t tri_stream;                    // where the fused triangulation runs (the context's side stream when there is one)
   const void *d_valid, *d_cnt, *d_model;      // MVO_EPI_DEBUG
 };

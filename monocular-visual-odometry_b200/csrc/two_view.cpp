@@ -74,13 +74,7 @@ extern "C" int mvo_estimate_relative_poses(mvo_ctx *ctx, const float *pts_img1, 
   }
   // ---- change of frame, after everything else (:114-118): basics::invRt ----
   if (!motion_cam2_to_cam1)
-    for (int s = 0; s < sol->num_solutions; ++s) {
-      double Rt[9], tt[3];
-      for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rt[i * 3 + j] = sol->R[s][j * 3 + i];
-      for (int i = 0; i < 3; ++i) tt[i] = -(Rt[i * 3] * sol->t[s][0] + Rt[i * 3 + 1] * sol->t[s][1] + Rt[i * 3 + 2] * sol->t[s][2]);
-      memcpy(sol->R[s], Rt, 72);
-      memcpy(sol->t[s], tt, 24);
-    }
+    for (int s = 0; s < sol->num_solutions; ++s) inv_rt(sol->R[s], sol->t[s]);
   // ---- choose a solution (:134-154); the score functions prune copies of the inlier lists, as in the reference ----
   int ne2 = n_e, nh2 = n_h;
   MVO_TRY(mvo_check_essential_score(sol->E, K, pts_img1, pts_img2, n, inl_e.data(), &ne2, 1.0, &sol->score_e));

@@ -1,8 +1,9 @@
 // The combine step of mvo_estimate_relative_poses_batch_dev (mvo.h): what mvo_estimate_relative_poses (two_view.cpp) does on the
 // host once its two RANSACs have returned, for every pair of a batch in one launch, one CTA per pair:
-//   cv::decomposeHomographyMat(H, K) + t /= |t|      epipolar.cu mvo_epi_homography_end (reference epipolar_geometry.cpp:119-126)
+//   cv::decomposeHomographyMat(H, K) + t /= |t|      epi::homography_motions, as mvo_epi_homography_end (epipolar_geometry.cpp:119-126)
 //   removeWrongRtOfHomography                        epi::filter_homography_solutions (epipolar_geometry.cpp:59-88)
-//   the solutions, their inlier rows, basics::invRt  two_view.cpp (motion_estimation.cpp:75-118)
+//   the solutions, their inlier rows                 two_view.cpp (motion_estimation.cpp:75-112)
+//   basics::invRt                                    inv_rt (mvo_internal.h), as two_view.cpp (motion_estimation.cpp:114-118)
 //   checkEssentialScore / checkHomographyScore       eh_scores.cuh, sigma = 1 (motion_estimation.cpp:501-664)
 //   the E / H choice                                 epi::eh_choose with mvo_params::eh_ratio_threshold (:134-154)
 // The host path runs all of this in g++ code for x86-64, which has no fused multiply-add.  This translation unit is compiled
@@ -60,20 +61,8 @@ __global__ void __launch_bounds__(RPC_T) k_relative_poses_combine(const MvoRelPo
     for (int q = 0; q < 3; ++q) sol.t[0][q] = er.t[q];
     S.ns = 0;
     if (n_h > 0) {
-      // mvo_epi_homography_end: Hn = K^-1 H K, decomposition, t /= |t| (a pure rotation keeps t = 0)
       for (int q = 0; q < 9; ++q) sol.H[q] = hd[q];
-      const double fx = a.K[0], fy = a.K[4], cx = a.K[2], cy = a.K[5];
-      const double Km[9] = {fx, 0, cx, 0, fy, cy, 0, 0, 1}, Ki[9] = {1 / fx, 0, -cx / fx, 0, 1 / fy, -cy / fy, 0, 0, 1};
-      double T[9], Hn[9];
-      epi::mat3_mul(sol.H, Km, T);
-      epi::mat3_mul(Ki, T, Hn);
-      const int ns = epi::decompose_homography(Hn, S.Rh, S.th, S.nh);
-      for (int s = 0; s < ns; ++s) {
-        double *ts = S.th + 3 * s;
-        const double nt = sqrt(ts[0] * ts[0] + ts[1] * ts[1] + ts[2] * ts[2]);
-        if (nt > 0) for (int q = 0; q < 3; ++q) ts[q] /= nt;
-      }
-      S.ns = ns;
+      S.ns = epi::homography_motions(sol.H, a.K, S.Rh, S.th, S.nh);
     }
     for (int s = 0; s < 4; ++s) S.keep[s] = 1;
   }
@@ -109,13 +98,7 @@ __global__ void __launch_bounds__(RPC_T) k_relative_poses_combine(const MvoRelPo
       for (int q = 0; q < 3; ++q) rt[12 * s + 9 + q] = sol.t[s][q];
     }
     if (!a.motion_cam2_to_cam1)                    // basics::invRt, after everything else (:114-118)
-      for (int s = 0; s < sol.num_solutions; ++s) {
-        double Rt[9], tt[3];
-        for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Rt[i * 3 + j] = sol.R[s][j * 3 + i];
-        for (int i = 0; i < 3; ++i) tt[i] = -(Rt[i * 3] * sol.t[s][0] + Rt[i * 3 + 1] * sol.t[s][1] + Rt[i * 3 + 2] * sol.t[s][2]);
-        for (int q = 0; q < 9; ++q) sol.R[s][q] = Rt[q];
-        for (int q = 0; q < 3; ++q) sol.t[s][q] = tt[q];
-      }
+      for (int s = 0; s < sol.num_solutions; ++s) inv_rt(sol.R[s], sol.t[s]);
     double Ki[9];
     epi::inv3(a.K, Ki);                            // the call checked that K inverts
     epi::essential_score_F(sol.E, Ki, S.F);

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE (CPU tier): the two-view kernels (csrc/epipolar_kernels.cuh — essential matrix, triangulation,
 // homography) built for the host with tests/cpp/cuda_emu.h and launched the way csrc/epipolar.cu launches them
 // (mvo_esti_motion_by_essential, mvo_esti_motion_by_homography, mvo_do_triangulation: the batch kernels with one pair and
-// cap = n, same thresholds, same post-processing).  The essential-matrix kernels have run on hardware; the homography kernels have not — this is their
+// cap = n, same thresholds, recoverPose's pick by the same epi::recover_pose_pick).  The essential-matrix kernels have run on hardware; the homography kernels have not — this is their
 // first execution of any kind.
 #include "cuda_emu.h"
 
@@ -30,17 +30,7 @@ int emu_essential(const float *p1, const float *p2, int n, const double *K, doub
   run_clusters(EFIN_C, EFIN_C, EFIN_T, sizeof(EpiFinSmem),
                [&] { k_epi_finish_batch(p1, p2, pn, n, cam, thr2, H, Es.data(), counts.data(), out.data(), oi.data(), inliers); });
   run_grid((unsigned)((n + 63) / 64), 1, 1, 256, 0, [&] { k_epi_vote_batch(p1, p2, pn, n, cam, out.data(), oi.data(), inliers); });
-  // recoverPose's choice on the host, as mvo_esti_motion_by_essential does it: the first candidate whose vote count is a maximum
-  const int32_t *g = oi.data() + 8;
-  int pick = 3;
-  if (g[0] >= g[1] && g[0] >= g[2] && g[0] >= g[3]) pick = 0;
-  else if (g[1] >= g[0] && g[1] >= g[2] && g[1] >= g[3]) pick = 1;
-  else if (g[2] >= g[0] && g[2] >= g[1] && g[2] >= g[3]) pick = 2;
-  oi[2] = g[pick];
-  const double *tt = out.data() + 27, sg = pick < 2 ? 1.0 : -1.0;
-  const double nt = sqrt(tt[0] * tt[0] + tt[1] * tt[1] + tt[2] * tt[2]);
-  memcpy(E, out.data(), 72); memcpy(R, out.data() + ((pick & 1) ? 18 : 9), 72);
-  for (int q = 0; q < 3; ++q) t[q] = sg * tt[q] / nt;
+  oi[2] = epi::recover_pose_pick(out.data(), oi.data() + 8, E, R, t);
   memcpy(out_i, oi.data(), 5 * sizeof(int32_t));
   if (getenv("MVO_EPI_DEBUG")) fprintf(stderr, "emu_essential: n %d inliers %d GN iterations %d\n", n, oi[0], oi[5]);
   return oi[0];
