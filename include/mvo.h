@@ -566,6 +566,60 @@ int mvo_vo_init_candidates_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, c
                                      const double *T_w_c_ref, const mvo_vo_params *vp, mvo_init_candidate_result *d_out,
                                      mvo_dmatch *d_kept, float *d_kept_pts3d, double *d_kept_angles);
 
+/* The new map points of the state machine's keyframe branch (vo_addFrame.cpp:93-124: helperFindInlierMatchesByEpipolarCons,
+ * helperTriangulatePoints with the known motion, retainGoodTriangulationResult_, pushCurrPointsToMap_) for the matched frame
+ * pairs of a batch, entirely on the device: the step after mvo_esti_motion_by_essential_batch_dev.  Pair p = (query frame, train
+ * frame) is (reference keyframe, current frame), as matchFeatures(ref_->descriptors_, curr_->descriptors_); its record says what
+ * the state machine computes when that frame is inserted as a keyframe with those two poses:
+ *   the essential RANSAC's inlier matches (img_idx = -1), the known motion T_curr_to_prev = T_w_c_curr^-1 * T_w_c_ref
+ *   (getMotionFromFrame1to2), the inliers triangulated with it on pixel2CamNormPlane points as mvo_do_triangulation does and moved
+ *   into the current camera (transCoord), retainGoodTriangulationResult_ (angles, their median, the drop by angle), and for every
+ *   kept point the map point's world position (preTranslatePoint3f with T_w_c_curr) and unit viewing direction (pos - camera
+ *   centre, normalised).
+ * Inputs: d_kpts / d_counts / batch / cap / d_pairs / n_pairs / d_matches / d_n_matches exactly as given to
+ * mvo_esti_motion_by_essential_batch_dev, and what it wrote (d_ess, d_ess_inliers; its d_pts3d is not needed and may have been
+ * NULL).  d_T_w_c: batch x 16 doubles on the device, each frame's camera->world pose (row-major), indexed like d_kpts.  K: host
+ * 3x3.  vp: host, the fields min_triang_angle and max_ratio_angle_to_median.
+ * Outputs of pair p: d_out[p]; inliers_matches_for_3d_ at d_kept + p * cap, inliers_pts3d_ (current camera) at d_kept_pts3d +
+ * p * cap * 3, triangulation_angles_of_inliers_ at d_kept_angles + p * cap, and optionally (NULL: not written) the world positions
+ * at d_kept_world + p * cap * 3 and the viewing directions at d_kept_norm + p * cap * 3, n_kept of each in the reference's order;
+ * nothing past n_kept is written, with one exception: the d_kept_pts3d row holds the pair's triangulated inliers between the
+ * second and the third launch (the call has no scratch memory of its own), so its entries n_kept .. n_inliers - 1 are left
+ * unspecified; nothing past n_inliers is written there.  A position and a direction are written for every kept point: whether the reference keypoint
+ * already has a map point (which the reference then reuses) is a question for the caller's map.
+ * Per pair: an essential status MVO_ERR_DEGENERATE gives usable = 0 and status MVO_OK (insert_keyframe returns before adding the
+ * keyframe); any other non-MVO_OK status is propagated.  MVO_ERR_INVALID_ARG for that pair alone, checked before anything is read
+ * through the value checked: a frame index outside [0, batch), d_n_matches[p] outside [0, cap] (both also for a degenerate
+ * pair), and for a pair whose essential status is MVO_OK n_inliers outside [0, d_n_matches[p]], an inlier index outside
+ * [0, d_n_matches[p]), a keypoint index of an inlier match outside its frame, a non-finite entry in either frame's pose.  A failed
+ * pair writes its status only.
+ * Numerics: the triangulation is the device's own (the arithmetic of mvo_do_triangulation); everything the state machine computes
+ * on the host is restated in the host's order of operations, without contraction.  Each angle uses the device's acos (2 ulp),
+ * the one step that is not the host's (glibc) bit for bit: the angles and median_angle are within a few ulp of the state
+ * machine's, and everything else is byte-identical unless an angle lies that close to a threshold.  A NaN angle, median_angle or
+ * direction has x86-64's default NaN bits.
+ * MVO_ERR_INVALID_ARG: a null required pointer, fx or fy not finite and > 0, a vp threshold that is not finite, batch or cap < 1,
+ * n_pairs < 0.  MVO_ERR_UNSUPPORTED: cap > 6400 or n_pairs > 65535 (the limits of mvo_esti_motion_by_essential_batch_dev), or a
+ * library built without the kernels' translation unit.  Asynchronous on the context stream: three kernel launches whatever
+ * n_pairs is (the checks and the known motion, the triangulation, the retain step and the map points), no host
+ * synchronisation, no scratch memory of the context (see d_kept_pts3d). */
+typedef struct mvo_keyframe_points_result {
+  int32_t status;      /* MVO_OK, or the pair's mvo_status */
+  int32_t usable;      /* 0: the essential RANSAC was degenerate, the state machine inserts no keyframe */
+  int32_t n_matches;   /* matches_with_ref_ (mvo_vo_frame_info::kf_matches) */
+  int32_t n_inliers;   /* inliers_matches_with_ref_ */
+  int32_t n_kept;      /* inliers_matches_for_3d_ (mvo_vo_frame_info::kf_new_points) */
+  int32_t pad;
+  double median_angle;                        /* retainGoodTriangulationResult_'s median (element n / 2); 0 when n_inliers = 0 */
+  double R_curr_to_prev[9], t_curr_to_prev[3];   /* the known motion the triangulation used */
+} mvo_keyframe_points_result;
+int mvo_vo_keyframe_points_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                     const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches, const int32_t *d_n_matches,
+                                     const mvo_two_view_result *d_ess, const int32_t *d_ess_inliers, const double *d_T_w_c,
+                                     const double *K, const mvo_vo_params *vp, mvo_keyframe_points_result *d_out,
+                                     mvo_dmatch *d_kept, float *d_kept_pts3d, double *d_kept_angles, float *d_kept_world,
+                                     double *d_kept_norm);
+
 typedef struct mvo_vo_frame_info {
   int32_t frame_id, state_in, state_out;   /* states: 0 BLANK, 1 DOING_INITIALIZATION, 2 DOING_TRACKING (vo.h:52-58) */
   int32_t keyframe;                        /* this frame became a keyframe */

@@ -356,6 +356,15 @@ extern "C" int mvo_esti_motion_by_essential_batch_dev(mvo_ctx *ctx, const mvo_ke
   return MVO_OK;
 }
 
+// declared in mvo_internal.h: the triangulation of mvo_vo_keyframe_points_batch_dev (its other two launches are in vo_init_batch.cu)
+int mvo_kf_triangulate_launch(mvo_ctx *ctx, const MvoKeyframePoints &a) {
+  { KTimer kt(ctx, KC_EPI);
+  k_kf_triangulate<<<dim3((a.cap + 127) / 128, a.n_pairs), 128, 0, ctx->stream>>>(a.kpts, (const int2 *)a.pairs, a.matches, a.ess_inliers, a.out,
+                                                                                 a.cap, a.fx, a.fy, a.cx, a.cy, a.kept_pts3d); }
+  MVO_CHECK_LAUNCH(ctx);
+  return MVO_OK;
+}
+
 // The combine step lives in two_view_batch.cu, a translation unit of its own that is compiled without contraction (Makefile).
 // libmvo.so always links it; a library assembled from a subset of the units without it reports MVO_ERR_UNSUPPORTED for the call.
 int mvo_relative_poses_combine(mvo_ctx *ctx, const MvoRelPosesCombine &a) __attribute__((weak));

@@ -572,6 +572,28 @@ k_triangulate_batch(const float *__restrict__ np1, const float *__restrict__ np2
   epi_triangulate_one(np1 + op * 2, np2 + op * 2, inl[op + j], Rt, out + op * 3, j);
 }
 
+// mvo_vo_keyframe_points_batch_dev, launch 2 of 3: doTriangulation of every usable pair's essential inliers with the known motion
+// that k_kf_motion (vo_init_batch.cu) put in the pair's record, on the pixel2CamNormPlane points of insert_keyframe; row j of the
+// pair's kept_pts3d row holds inlier j afterwards.  k_kf_motion has checked every index read here.
+__global__ void __launch_bounds__(128)
+k_kf_triangulate(const mvo_keypoint *__restrict__ kpts, const int2 *__restrict__ pairs, const mvo_dmatch *__restrict__ matches,
+                 const int32_t *__restrict__ inl, const mvo_keyframe_points_result *__restrict__ res, int cap, double fx, double fy,
+                 double cx, double cy, float *__restrict__ out) {
+  const int pair = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  const mvo_keyframe_points_result &r = res[pair];
+  if (r.status != MVO_OK || r.usable != 1 || j >= r.n_inliers) return;
+  double Rt[12];
+  for (int q = 0; q < 9; ++q) Rt[q] = r.R_curr_to_prev[q];
+  for (int q = 0; q < 3; ++q) Rt[9 + q] = r.t_curr_to_prev[q];
+  const size_t op = (size_t)pair * cap;
+  const int2 fr = pairs[pair];
+  const mvo_dmatch m = matches[op + inl[op + j]];
+  const mvo_keypoint kq = kpts[(size_t)fr.x * cap + m.query_idx], kt = kpts[(size_t)fr.y * cap + m.train_idx];
+  const float np1[2] = {(float)(((double)kq.x - cx) / fx), (float)(((double)kq.y - cy) / fy)};
+  const float np2[2] = {(float)(((double)kt.x - cx) / fx), (float)(((double)kt.y - cy) / fy)};
+  epi_triangulate_one(np1, np2, 0, Rt, out + op * 3, j);
+}
+
 // ---------------------------------------------------------------------------------------------------- homography
 // estiMotionByHomography (reference src/geometry/epipolar_geometry.cpp:90-128): cv::findHomography(pts1, pts2, RANSAC,
 // 3.0, mask) + H /= H(2,2) + inliers from the mask + cv::decomposeHomographyMat(H, K) + t /= |t|.  Same batched design

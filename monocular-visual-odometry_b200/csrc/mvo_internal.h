@@ -136,7 +136,7 @@ int mvo_reserve(mvo_ctx *ctx, DevBuf &b, size_t bytes);
 int mvo_reserve_pinned(mvo_ctx *ctx, PinBuf &b, size_t bytes);
 
 // Host arithmetic on rigid transforms (4x4 row-major doubles) shared by the tracker and the VO state machine, in the reference's
-// operation order: tracker.cpp and vo_pipeline.cpp get the same bits.  inv_rigid and rt_to_T also serve vo_init_batch.cu, which
+// operation order: tracker.cpp and vo_pipeline.cpp get the same bits.  inv_rigid, rt_to_T and pre_translate also serve vo_init_batch.cu, which
 // is compiled without contraction and so gets the host's bits as well.
 #if defined(__CUDACC__)
 #define MVO_HD __host__ __device__
@@ -172,7 +172,7 @@ static inline MVO_HD void rt_to_T(const double *R, const double *t, double *T) {
   T[12] = T[13] = T[14] = 0; T[15] = 1;
 }
 // basics::preTranslatePoint3f: T(row, j) * p[j] accumulated in double over j = 0..3, narrowed to Point3f
-static inline void pre_translate(const float *p, const double *T, float *out) {
+static inline MVO_HD void pre_translate(const float *p, const double *T, float *out) {
   const double p0 = p[0], p1 = p[1], p2 = p[2];
   for (int r = 0; r < 3; ++r) {
     double a = 0;
@@ -394,6 +394,25 @@ struct MvoInitCandidates {
   double *kept_angles;
 };
 int mvo_vo_init_candidates_launch(mvo_ctx *ctx, const MvoInitCandidates &a);
+// mvo_vo_keyframe_points_batch_dev (vo_pipeline.cpp checks the arguments): the checks and the known motion, and the retain step
+// with the map points, are launched by vo_init_batch.cu (one CTA per pair each); between them the triangulation
+// (mvo_kf_triangulate_launch, epipolar.cu) writes pair p's triangulated inliers into its kept_pts3d row, which the last kernel
+// stages before it overwrites the row with the kept points
+struct MvoKeyframePoints {
+  const mvo_keypoint *kpts;
+  const int32_t *counts, *pairs, *n_matches, *ess_inliers;
+  const mvo_dmatch *matches;
+  const mvo_two_view_result *ess;
+  const double *T_w_c;
+  int batch, cap, n_pairs;
+  double fx, fy, cx, cy, min_triang_angle, max_ratio_angle_to_median;
+  mvo_keyframe_points_result *out;
+  mvo_dmatch *kept;
+  float *kept_pts3d, *kept_world;
+  double *kept_angles, *kept_norm;
+};
+int mvo_vo_keyframe_points_launch(mvo_ctx *ctx, const MvoKeyframePoints &a);
+int mvo_kf_triangulate_launch(mvo_ctx *ctx, const MvoKeyframePoints &a);
 cudaStream_t mvo_side_stream(mvo_ctx *ctx);      // a second non-blocking stream of the context, created on first use (ctx.cu)
 int mvo_epi_essential_ex(mvo_ctx *ctx, const float *pts1, const float *pts2, int n, const double *K, double threshold,
                          double *E, double *R, double *t, int32_t *inliers, int *n_inliers, int want_pose,

@@ -1026,3 +1026,40 @@ extern "C" int mvo_vo_init_candidates_batch_dev(mvo_ctx *ctx, const mvo_keypoint
   a.out = d_out; a.kept = d_kept; a.kept_pts3d = d_kept_pts3d; a.kept_angles = d_kept_angles;
   return mvo_vo_init_candidates_launch(ctx, a);
 }
+
+// The first and last kernels of mvo_vo_keyframe_points_batch_dev live in vo_init_batch.cu as well (the triangulation between them
+// in epipolar.cu); a library without that unit reports MVO_ERR_UNSUPPORTED for the call.
+int mvo_vo_keyframe_points_launch(mvo_ctx *ctx, const MvoKeyframePoints &a) __attribute__((weak));
+
+// mvo_vo_keyframe_points_batch_dev (mvo.h): the call-level checks here, everything per pair in three launches
+extern "C" int mvo_vo_keyframe_points_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const int32_t *d_counts, int batch, int cap,
+                                                const int32_t *d_pairs, int n_pairs, const mvo_dmatch *d_matches,
+                                                const int32_t *d_n_matches, const mvo_two_view_result *d_ess,
+                                                const int32_t *d_ess_inliers, const double *d_T_w_c, const double *K,
+                                                const mvo_vo_params *vp, mvo_keyframe_points_result *d_out, mvo_dmatch *d_kept,
+                                                float *d_kept_pts3d, double *d_kept_angles, float *d_kept_world, double *d_kept_norm) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (!d_kpts || !d_counts || !d_pairs || !d_matches || !d_n_matches || !d_ess || !d_ess_inliers || !d_T_w_c || !K || !vp || !d_out ||
+      !d_kept || !d_kept_pts3d || !d_kept_angles)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo keyframe points batch: null pointer");
+  if (!mvo_vo_keyframe_points_launch)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "vo keyframe points batch: the library was built without vo_init_batch.cu");
+  if (n_pairs < 0 || batch < 1 || cap < 1)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo keyframe points batch: n_pairs=%d batch=%d cap=%d", n_pairs, batch, cap);
+  if (!(std::isfinite(K[0]) && K[0] > 0 && std::isfinite(K[4]) && K[4] > 0))
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo keyframe points batch: fx and fy must be finite and positive");
+  if (!std::isfinite(vp->min_triang_angle) || !std::isfinite(vp->max_ratio_angle_to_median))
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "vo keyframe points batch: a threshold of vp is not finite");
+  if (cap > 6400) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "vo keyframe points batch: cap %d above 6400 correspondences", cap);
+  if (n_pairs > 65535) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "vo keyframe points batch: %d pairs, at most 65535 per call", n_pairs);
+  if (n_pairs == 0) return MVO_OK;
+  MvoKeyframePoints a;
+  a.kpts = d_kpts; a.counts = d_counts; a.pairs = d_pairs; a.n_matches = d_n_matches; a.ess_inliers = d_ess_inliers; a.matches = d_matches;
+  a.ess = d_ess; a.T_w_c = d_T_w_c;
+  a.batch = batch; a.cap = cap; a.n_pairs = n_pairs;
+  a.fx = K[0]; a.fy = K[4]; a.cx = K[2]; a.cy = K[5];
+  a.min_triang_angle = vp->min_triang_angle; a.max_ratio_angle_to_median = vp->max_ratio_angle_to_median;
+  a.out = d_out; a.kept = d_kept; a.kept_pts3d = d_kept_pts3d; a.kept_world = d_kept_world; a.kept_angles = d_kept_angles;
+  a.kept_norm = d_kept_norm;
+  return mvo_vo_keyframe_points_launch(ctx, a);
+}

@@ -40,6 +40,11 @@ INIT_CANDIDATE_RESULT_DTYPE = np.dtype(
      ("normalized", "<i4"), ("pad", "<i4"), ("scale", "<f8"), ("mean_pixel_dist", "<f8"), ("median_angle", "<f8"),
      ("t_curr_to_prev", "<f8", (3,)), ("T_w_c", "<f8", (16,))])
 assert INIT_CANDIDATE_RESULT_DTYPE.itemsize == 208
+# mvo_keyframe_points_result (vo_keyframe_points_batch_dev): one record per frame pair
+KEYFRAME_POINTS_RESULT_DTYPE = np.dtype(
+    [("status", "<i4"), ("usable", "<i4"), ("n_matches", "<i4"), ("n_inliers", "<i4"), ("n_kept", "<i4"), ("pad", "<i4"),
+     ("median_angle", "<f8"), ("R_curr_to_prev", "<f8", (9,)), ("t_curr_to_prev", "<f8", (3,))])
+assert KEYFRAME_POINTS_RESULT_DTYPE.itemsize == 128
 
 MVO_OK = 0
 ERR_NAMES = {0: "MVO_OK", -1: "MVO_ERR_INVALID_ARG", -2: "MVO_ERR_NO_DEVICE", -3: "MVO_ERR_CUDA",
@@ -182,6 +187,8 @@ SIGNATURES = {
     "mvo_vo_frame_data": (_i, [_vp, _i, _i, _vp, _i, _pi]),
     "mvo_vo_init_candidates_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(VoParams), _vp, _vp, _vp,
                                               _vp]),
+    "mvo_vo_keyframe_points_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(VoParams), _vp, _vp,
+                                              _vp, _vp, _vp, _vp]),
     "mvo_vo_has_keyframe": (_i, [_vp, _i]),
     "mvo_write_pose_file": (_i, [C.c_char_p, _vp, _i]),
     "mvo_read_pose_file": (_i, [C.c_char_p, _vp, _i, _pi]),
@@ -361,6 +368,20 @@ class Context:
                                                             _ptr(d_matches), _ptr(d_n_matches), _ptr(d_rp), _ptr(d_rp_inliers),
                                                             _ptr(d_rp_pts3d), _ptr(T), C.byref(vo_params), _ptr(d_out), _ptr(d_kept),
                                                             _ptr(d_kept_pts3d), _ptr(d_kept_angles)))
+
+    def vo_keyframe_points_batch_dev(self, d_kpts, d_counts, batch, cap, d_pairs, n_pairs, d_matches, d_n_matches, d_ess, d_ess_inliers,
+                                     d_T_w_c, K, vo_params, d_out, d_kept, d_kept_pts3d, d_kept_angles, d_kept_world=None, d_kept_norm=None):
+        """The new map points of the state machine's keyframe branch for every (reference keyframe, frame) pair of an
+        esti_motion_by_essential_batch_dev call, triangulated with the known motion T_w_c_curr^-1 * T_w_c_ref of the frames' poses
+        (d_T_w_c: batch x 16 doubles on the device).  All device pointers except K (host 3x3) and vo_params (VoParams): pair p's
+        KEYFRAME_POINTS_RESULT_DTYPE record in d_out[p], its kept matches at d_kept + p * cap, kept points (current camera) at
+        d_kept_pts3d + p * cap * 3, kept angles at d_kept_angles + p * cap and, when given, the map points' world positions at
+        d_kept_world + p * cap * 3 and viewing directions at d_kept_norm + p * cap * 3."""
+        K = _c(K, np.float64)
+        self._chk(self.lib.mvo_vo_keyframe_points_batch_dev(self.h, _ptr(d_kpts), _ptr(d_counts), batch, cap, _ptr(d_pairs), n_pairs,
+                                                            _ptr(d_matches), _ptr(d_n_matches), _ptr(d_ess), _ptr(d_ess_inliers),
+                                                            _ptr(d_T_w_c), _ptr(K), C.byref(vo_params), _ptr(d_out), _ptr(d_kept),
+                                                            _ptr(d_kept_pts3d), _ptr(d_kept_angles), _ptr(d_kept_world), _ptr(d_kept_norm)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):
