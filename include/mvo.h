@@ -619,6 +619,47 @@ int mvo_vo_keyframe_points_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, c
                                      const double *K, const mvo_vo_params *vp, mvo_keyframe_points_result *d_out,
                                      mvo_dmatch *d_kept, float *d_kept_pts3d, double *d_kept_angles, float *d_kept_world,
                                      double *d_kept_norm);
+/* The first step of the state machine's tracking branch (poseEstimationPnP_) for many frames at once, entirely on the device:
+ * for every job (frame, guess pose) what pose_estimation_pnp computes before solvePnPRansac — getMappointsInCurrentView_, the
+ * match of the map points in view against the frame (matchFeatures with the tracking method and radius, xiang_gao_ratio /
+ * lowe_ratio of the context) and the 3D-2D pairs.  The batched PnP is not part of this call.
+ * Inputs: d_kpts / d_desc / d_counts / batch / cap in the layout of mvo_orb_extract_batch_dev; d_frames: n_jobs int32 frame
+ * indices; d_T_w_c_guess: n_jobs x 16 doubles, the guess pose of each job (camera->world, row-major; the state machine uses the
+ * reference keyframe's pose); d_map_pts / d_map_desc: one map, n_map points (float x, y, z) and descriptors, whose position is
+ * the map index (the state machine's container order, as mvo_vo_get_map returns it).  K: host 3x3; rows / cols: the image size
+ * of the inside test; method_index / radius: mvo_vo_params::track.match_method / match_radius.
+ * Job j: T_c_w = inverse of the guess; every map point in index order is projected (preTranslatePoint3f, z < 0 rejected,
+ * cam2pixel) and kept when 0 < u < cols and 0 < v < rows; the candidates, in map order, are matched as the query set of
+ * mvo_match_features against the frame's keypoints (method 3: candidate pixels against keypoint pts within radius).
+ * Outputs of job j (nothing past a count is written):
+ *   d_out[j]; d_cand + j * n_map: the candidates' map indices (n_candidates); d_cand_xy + j * n_map * 2: their projected pixels
+ *   (optional, NULL: not written); d_matches + j * cap: matches_with_map_, byte-identical to what the state machine's matcher
+ *   returns (query_idx = rank in the candidate list, train_idx = keypoint); d_pts3d + j * cap * 3 / d_pts2d + j * cap * 2: the map
+ *   point and keypoint pt of every match, the solvePnPRansac inputs (optional, NULL: not written; both or neither).
+ * Per job: no candidates, no keypoints, or method 2 with fewer than 2 keypoints: status MVO_OK with 0 matches (the state machine
+ * skips the matcher there).  Counts are clamped to [0, cap].  MVO_ERR_INVALID_ARG for that job alone: a frame index outside
+ * [0, batch), a non-finite entry of its guess pose.  MVO_ERR_UNSUPPORTED for that job alone when the device filter cannot finish
+ * it: more map points in view pass the distance threshold than the filter's capacity (2048 up to 8192, the power of two that
+ * covers cap and n_map), or libstdc++'s introsort would heapsort at its depth limit; the state machine would still produce a
+ * match list for such a frame.  A failed job writes its status only.
+ * MVO_ERR_INVALID_ARG: a null required pointer (d_desc, d_counts, d_frames, d_T_w_c_guess, K, d_out, d_cand, d_matches, and
+ * d_map_pts / d_map_desc when n_map > 0, d_kpts for method 3 or with d_pts2d), fx or fy not finite and > 0, rows or cols < 1, a method index outside
+ * 1..3, batch or cap < 1, n_jobs or n_map < 0, only one of d_pts3d / d_pts2d.  MVO_ERR_UNSUPPORTED: cap > 8192, n_map > 65535,
+ * n_jobs > 65535, n_jobs * n_map > 2^26 (the matcher keys of every job).  Asynchronous on the context stream: methods 1 and 2
+ * make two kernel launches (the matcher of every map point against every job's frame, then the filter, which projects the
+ * map), method 3 three (the projection first: the radius gate needs the pixels), whatever n_jobs is; n_map = 0 makes one (the
+ * filter) and n_jobs = 0 none.  No host synchronisation once the context's scratch has reached its size. */
+typedef struct mvo_map_matches_result {
+  int32_t status;        /* MVO_OK, or the job's mvo_status */
+  int32_t n_candidates;  /* map points in view (mvo_vo_frame_info::n_candidates) */
+  int32_t n_matches;     /* matches_with_map_ before PnP (mvo_vo_frame_info::n_matches) */
+  int32_t pad;
+} mvo_map_matches_result;
+int mvo_vo_map_matches_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts, int batch,
+                                 int cap, const int32_t *d_frames, const double *d_T_w_c_guess, int n_jobs, const float *d_map_pts,
+                                 const uint8_t *d_map_desc, int n_map, const double *K, int rows, int cols, int method_index,
+                                 float radius, mvo_map_matches_result *d_out, int32_t *d_cand, float *d_cand_xy, mvo_dmatch *d_matches,
+                                 float *d_pts3d, float *d_pts2d);
 
 typedef struct mvo_vo_frame_info {
   int32_t frame_id, state_in, state_out;   /* states: 0 BLANK, 1 DOING_INITIALIZATION, 2 DOING_TRACKING (vo.h:52-58) */

@@ -170,6 +170,9 @@ match_kernel(const uint4 *__restrict__ d1, const float2 *__restrict__ xy1, int n
 // and streams them through shared memory kMaxChunk at a time, so that a batch with many pairs can use one split per tile and
 // skip the merge.  Tiles beyond a pair's query count and splits beyond its train count exit; pairs with a frame index outside
 // [0, batch) (and method-2 pairs with fewer than two trains) are left to the tail kernel, which reports them.
+// kMapQuery (mvo_vo_map_matches_batch_dev): the queries are one map's descriptors, shared by every job, and the trains are frame
+// frames[z] of job z; MODE 2 takes job z's query pixels from qxy.  Keys and partial winners are then laid out per job with n_map
+// query rows instead of cap.
 struct MatchBatchArgs {
   const uint4 *desc;             // [batch][cap][2]
   const mvo_keypoint *kpts;      // [batch][cap] (MODE 2: pt)
@@ -180,9 +183,14 @@ struct MatchBatchArgs {
   uint32_t *part;                // [n_pairs][gridDim.y][cap][W] partial winners
   unsigned int *tickets;         // [n_pairs][gridDim.x], zero between launches
   uint32_t *keys;                // [n_pairs][cap][W]
+  // kMapQuery only
+  const uint4 *qdesc;            // [n_map][2]
+  const float2 *qxy;             // [n_jobs][n_map] (MODE 2)
+  const int32_t *frames;         // [n_jobs]
+  int nq;                        // n_map
 };
 
-template <int MODE>
+template <int MODE, bool kMapQuery = false>
 __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
   pdl_wait();                              // the extraction wrote descriptors, keypoints and counts
   pdl_launch_dependents();
@@ -190,13 +198,20 @@ __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
   __shared__ float2 s_xy[MODE == 2 ? kMaxChunk : 1];
   __shared__ bool s_last;
   const int p = blockIdx.z;
-  const int2 pr = a.pairs[p];
-  if (pr.x < 0 || pr.x >= a.batch || pr.y < 0 || pr.y >= a.batch) return;
-  const int n1 = min(max(a.counts[pr.x], 0), a.cap), n2 = min(max(a.counts[pr.y], 0), a.cap);
+  int2 pr;
+  if (kMapQuery) {
+    pr = make_int2(0, a.frames[p]);
+    if (pr.y < 0 || pr.y >= a.batch) return;
+  } else {
+    pr = a.pairs[p];
+    if (pr.x < 0 || pr.x >= a.batch || pr.y < 0 || pr.y >= a.batch) return;
+  }
+  const int n1 = kMapQuery ? a.nq : min(max(a.counts[pr.x], 0), a.cap), n2 = min(max(a.counts[pr.y], 0), a.cap);
+  const int rows = kMapQuery ? a.nq : a.cap;           // query rows per pair in keys and part
   const int nsplit = (n2 + a.span - 1) / a.span;       // splits that hold trains of this pair
   const int split = blockIdx.y;
   if ((int)blockIdx.x * kQ >= n1 || split >= nsplit || (MODE == 1 && n2 < 2)) return;
-  const uint4 *d1 = a.desc + (size_t)pr.x * a.cap * 2, *d2 = a.desc + (size_t)pr.y * a.cap * 2;
+  const uint4 *d1 = kMapQuery ? a.qdesc : a.desc + (size_t)pr.x * a.cap * 2, *d2 = a.desc + (size_t)pr.y * a.cap * 2;
   const mvo_keypoint *k1 = a.kpts + (size_t)pr.x * a.cap, *k2 = a.kpts + (size_t)pr.y * a.cap;
 
   const int q = blockIdx.x * kQ + threadIdx.x;
@@ -208,7 +223,8 @@ __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
     uint4 u = d1[(size_t)qc * 2], v = d1[(size_t)qc * 2 + 1];
     qw[0] = u.x; qw[1] = u.y; qw[2] = u.z; qw[3] = u.w;
     qw[4] = v.x; qw[5] = v.y; qw[6] = v.z; qw[7] = v.w;
-    if (MODE == 2) { qx = k1[qc].x; qy = k1[qc].y; }
+    if (MODE == 2 && kMapQuery) { const float2 pt = a.qxy[(size_t)p * a.nq + qc]; qx = pt.x; qy = pt.y; }
+    else if (MODE == 2) { qx = k1[qc].x; qy = k1[qc].y; }
   }
 
   uint32_t b1 = 0xFFFFFFFFu, b2 = 0xFFFFFFFFu;
@@ -238,7 +254,7 @@ __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
   }
 
   constexpr int W = (MODE == 1) ? 2 : 1;
-  uint32_t *keys = a.keys + (size_t)p * a.cap * W;
+  uint32_t *keys = a.keys + (size_t)p * rows * W;
   if (nsplit == 1) {
     if (q < n1) {
       keys[(size_t)q * W] = b1;
@@ -246,10 +262,10 @@ __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
     }
     return;
   }
-  uint32_t *part = a.part + (size_t)p * gridDim.y * a.cap * W;
+  uint32_t *part = a.part + (size_t)p * gridDim.y * rows * W;
   if (q < n1) {
-    part[((size_t)split * a.cap + q) * W] = b1;
-    if (MODE == 1) part[((size_t)split * a.cap + q) * W + 1] = b2;
+    part[((size_t)split * rows + q) * W] = b1;
+    if (MODE == 1) part[((size_t)split * rows + q) * W + 1] = b2;
   }
   __threadfence();
   __syncthreads();
@@ -265,7 +281,7 @@ __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
   if (q < n1) {
     uint32_t m1 = 0xFFFFFFFFu, m2 = 0xFFFFFFFFu;
     for (int s = 0; s < nsplit; ++s) {
-      const uint32_t *pp = part + ((size_t)s * a.cap + q) * W;
+      const uint32_t *pp = part + ((size_t)s * rows + q) * W;
       const uint32_t x1 = __ldcg(pp);
       if (MODE == 1) {
         const uint32_t x2 = __ldcg(pp + 1);
@@ -280,17 +296,12 @@ __global__ void __launch_bounds__(kQ) match_batch_kernel(MatchBatchArgs a) {
   }
 }
 
-}  // namespace
-
-// match_batch_kernel over n_pairs pairs (mvo_internal.h); d_keys: [n_pairs][cap][W] (W = 2 for mode 1)
-int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
-                           int batch, int cap, const int32_t *d_pairs, int n_pairs, float radius, uint32_t *d_keys) {
-  if (mode < 0 || mode > 2) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "match batch: bad mode %d", mode);
-  if (cap < 1 || cap > 65535 || n_pairs > 65535)
-    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "match batch: cap=%d n_pairs=%d outside [1,65535]", cap, n_pairs);
-  if (n_pairs <= 0) return MVO_OK;
+// The grid, scratch and launch of match_batch_kernel for n_pairs pairs of `rows` query rows each (a.cap trains at most): everything
+// but the pair / job fields of a, which the caller has set.
+int match_batch_enqueue(mvo_ctx *ctx, int mode, bool map_query, MatchBatchArgs a, int rows, int n_pairs, float radius) {
   const int W = mode == 1 ? 2 : 1;
-  const int qtiles = (cap + kQ - 1) / kQ;
+  const int cap = a.cap;
+  const int qtiles = (rows + kQ - 1) / kQ;
   // The whole batch, not one pair, has to fill the SMs: about `waves` CTAs per SM over all pairs (the rule of the single-pair
   // launch above), so a pair gets waves * sm_count / (qtiles * n_pairs) splits, at least one and no shorter than 32 trains.
   // With a chunk loop in the CTA there is no upper bound on a split's length: 63 pairs of 2001 keypoints run unsplit
@@ -304,13 +315,11 @@ int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, c
   const int span = (cap + nsplit - 1) / nsplit;
   nsplit = (cap + span - 1) / span;
 
-  MatchBatchArgs a;
-  a.desc = (const uint4 *)d_desc; a.kpts = d_kpts; a.counts = d_counts; a.pairs = (const int2 *)d_pairs;
-  a.batch = batch; a.cap = cap; a.span = span;
+  a.span = span;
   a.r2 = radius * radius;   // feature_match.cpp:96
-  a.part = nullptr; a.tickets = nullptr; a.keys = d_keys;
+  a.part = nullptr; a.tickets = nullptr;
   if (nsplit > 1) {
-    MVO_TRY(mvo_reserve(ctx, ctx->matchb_part, (size_t)n_pairs * nsplit * cap * W * 4));
+    MVO_TRY(mvo_reserve(ctx, ctx->matchb_part, (size_t)n_pairs * nsplit * rows * W * 4));
     const size_t had = ctx->matchb_tickets.cap;
     MVO_TRY(mvo_reserve(ctx, ctx->matchb_tickets, (size_t)n_pairs * qtiles * 4));
     if (ctx->matchb_tickets.cap != had)    // a new block: zero once, the kernel leaves it zeroed
@@ -320,11 +329,47 @@ int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, c
   }
   dim3 grid(qtiles, nsplit, n_pairs), block(kQ);
   KTimer kt(ctx, KC_MATCH);
-  if (mode == 0) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<0>, a));
-  else if (mode == 1) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<1>, a));
-  else MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<2>, a));
+  if (map_query) {
+    if (mode == 0) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<0, true>, a));
+    else if (mode == 1) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<1, true>, a));
+    else MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<2, true>, a));
+  } else {
+    if (mode == 0) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<0>, a));
+    else if (mode == 1) MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<1>, a));
+    else MVO_CUDA(ctx, launch_pdl3(ctx->stream, grid, block, 0, match_batch_kernel<2>, a));
+  }
   MVO_CHECK_LAUNCH(ctx);
   return MVO_OK;
+}
+
+}  // namespace
+
+// match_batch_kernel over n_pairs pairs (mvo_internal.h); d_keys: [n_pairs][cap][W] (W = 2 for mode 1)
+int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                           int batch, int cap, const int32_t *d_pairs, int n_pairs, float radius, uint32_t *d_keys) {
+  if (mode < 0 || mode > 2) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "match batch: bad mode %d", mode);
+  if (cap < 1 || cap > 65535 || n_pairs > 65535)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "match batch: cap=%d n_pairs=%d outside [1,65535]", cap, n_pairs);
+  if (n_pairs <= 0) return MVO_OK;
+  MatchBatchArgs a = {};
+  a.desc = (const uint4 *)d_desc; a.kpts = d_kpts; a.counts = d_counts; a.pairs = (const int2 *)d_pairs;
+  a.batch = batch; a.cap = cap; a.keys = d_keys;
+  return match_batch_enqueue(ctx, mode, false, a, cap, n_pairs, radius);
+}
+
+// the map-query form (mvo_internal.h); d_keys: [n_jobs][n_map][W]
+int mvo_match_map_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                               int batch, int cap, const int32_t *d_frames, int n_jobs, const uint8_t *d_map_desc, int n_map,
+                               const float *d_qxy, float radius, uint32_t *d_keys) {
+  if (mode < 0 || mode > 2) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "match map batch: bad mode %d", mode);
+  if (cap < 1 || cap > 65535 || n_jobs > 65535 || n_map > 65535)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "match map batch: cap=%d n_jobs=%d n_map=%d outside [1,65535]", cap, n_jobs, n_map);
+  if (n_jobs <= 0 || n_map <= 0) return MVO_OK;
+  MatchBatchArgs a = {};
+  a.desc = (const uint4 *)d_desc; a.kpts = d_kpts; a.counts = d_counts;
+  a.batch = batch; a.cap = cap; a.keys = d_keys;
+  a.qdesc = (const uint4 *)d_map_desc; a.qxy = (const float2 *)d_qxy; a.frames = d_frames; a.nq = n_map;
+  return match_batch_enqueue(ctx, mode, true, a, n_map, n_jobs, radius);
 }
 
 int mvo_match_launch(mvo_ctx *ctx, int mode, const uint8_t *d_d1, const float *d_xy1, int n1,

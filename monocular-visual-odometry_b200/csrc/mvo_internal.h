@@ -101,6 +101,8 @@ struct mvo_ctx {
   PinBuf match_h;
   // batched matchFeatures (mvo_match_features_batch_dev): partial winners, merge tickets, packed keys of every pair
   DevBuf matchb_part, matchb_tickets, matchb_keys;
+  // mvo_vo_map_matches_batch_dev: every job's in-view flags, and its projected pixels for the radius-gated matcher (method 3)
+  DevBuf mapm_buf;
   // batched two-view calls (mvo_esti_motion_by_essential_batch_dev, mvo_estimate_relative_poses_batch_dev): points, hypotheses,
   // counts and finish outputs of every pair; its own block, so that it never aliases the single-pair jobs' buffers
   DevBuf epib_buf;
@@ -434,6 +436,11 @@ int mvo_match_launch_ndev(mvo_ctx *ctx, int mode, const uint8_t *d_d1, const flo
 // d_keys: [n_pairs][cap][W] packed keys, W = 2 for mode 1.  Pairs with an out-of-range frame are skipped
 int mvo_match_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
                            int batch, int cap, const int32_t *d_pairs, int n_pairs, float radius, uint32_t *d_keys);
+// the same with one map's descriptors (n_map) as the queries of every job and frame d_frames[j] as job j's trains; mode 2 reads job
+// j's query pixels at d_qxy + j * n_map * 2.  d_keys: [n_jobs][n_map][W].  Jobs with an out-of-range frame are skipped
+int mvo_match_map_batch_launch(mvo_ctx *ctx, int mode, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                               int batch, int cap, const int32_t *d_frames, int n_jobs, const uint8_t *d_map_desc, int n_map,
+                               const float *d_qxy, float radius, uint32_t *d_keys);
 // pnp.cu: device-resident solvePnPRansac replacement (see there)
 int mvo_pnp_dev_buffers(mvo_ctx *ctx, int n, float **p3, float **p2, double **pose_io, int32_t **out_i, int32_t **inl);
 int mvo_pnp_dev_run(mvo_ctx *ctx, int n, const double *K, const int32_t *d_n);

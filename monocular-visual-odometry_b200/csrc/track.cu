@@ -260,3 +260,67 @@ extern "C" int mvo_match_features_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_
   ctx->launches++;
   return MVO_OK;
 }
+
+// poseEstimationPnP_ up to solvePnPRansac for a batch of (frame, guess pose) jobs against one map (mvo.h): methods 1 / 2 launch the
+// map-query matcher (match.cu) and k_map_match_filter, which projects the map itself; method 3 projects first
+// (k_project_map_batch), because the matcher's radius gate needs the pixels.  A fixed number of launches whatever n_jobs is; no host
+// synchronisation once the scratch buffers have reached their size.
+extern "C" int mvo_vo_map_matches_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const uint8_t *d_desc, const int32_t *d_counts,
+                                            int batch, int cap, const int32_t *d_frames, const double *d_T_w_c_guess, int n_jobs,
+                                            const float *d_map_pts, const uint8_t *d_map_desc, int n_map, const double *K, int rows,
+                                            int cols, int method_index, float radius, mvo_map_matches_result *d_out, int32_t *d_cand,
+                                            float *d_cand_xy, mvo_dmatch *d_matches, float *d_pts3d, float *d_pts2d) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (method_index < 1 || method_index > 3)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "map matches batch: wrong method index %d", method_index);
+  if (batch < 1 || cap < 1 || n_jobs < 0 || n_map < 0 || rows < 1 || cols < 1)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "map matches batch: batch=%d cap=%d n_jobs=%d n_map=%d rows=%d cols=%d", batch, cap, n_jobs,
+                    n_map, rows, cols);
+  if (!d_desc || !d_counts || !d_frames || !d_T_w_c_guess || !K || !d_out || !d_cand || !d_matches ||
+      (n_map > 0 && (!d_map_pts || !d_map_desc)) || ((method_index == 3 || d_pts2d) && !d_kpts) || (!d_pts3d != !d_pts2d))
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "map matches batch: null pointer");
+  if (!(isfinite(K[0]) && K[0] > 0 && isfinite(K[4]) && K[4] > 0))
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "map matches batch: fx=%g fy=%g", K[0], K[4]);
+  if (cap > MF_MAXN) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "map matches batch: cap %d above the device filter's %d", cap, MF_MAXN);
+  if (n_map > 65535 || n_jobs > 65535 || (long long)n_jobs * n_map > (1ll << 26))
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "map matches batch: n_jobs=%d n_map=%d (at most 65535 each, 2^26 together)", n_jobs, n_map);
+  if (n_jobs == 0) return MVO_OK;
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int mode = method_index == 1 ? 0 : (method_index == 2 ? 1 : 2);
+  const int W = mode == 1 ? 2 : 1;
+  const size_t cells = (size_t)n_jobs * n_map;
+  const size_t vis_bytes = (cells + 15) / 16 * 16;
+  MVO_TRY(mvo_reserve(ctx, ctx->mapm_buf, vis_bytes + (mode == 2 ? cells * 8 : 0) + 16));
+  uint8_t *vis = (uint8_t *)ctx->mapm_buf.p;
+  float2 *xy = (float2 *)(vis + vis_bytes);
+  uint32_t *keys = nullptr;
+  if (n_map > 0) {
+    MVO_TRY(mvo_reserve(ctx, ctx->matchb_keys, cells * W * 4));
+    keys = (uint32_t *)ctx->matchb_keys.p;
+    if (mode == 2) {
+      KTimer kt(ctx, KC_TRACK);
+      MVO_CUDA(ctx, launch_pdl3(ctx->stream, dim3((n_map + 255) / 256, n_jobs), dim3(256), 0, k_project_map_batch, d_map_pts, n_map,
+                                d_T_w_c_guess, K[0], K[4], K[2], K[5], (float)cols, (float)rows, xy));
+      ctx->launches++;
+    }
+    MVO_TRY(mvo_match_map_batch_launch(ctx, mode, d_kpts, d_desc, d_counts, batch, cap, d_frames, n_jobs, d_map_desc, n_map,
+                                       (const float *)xy, radius, keys));
+  }
+  // the filter's capacity covers the frame capacity and, up to MF_MAXN, every map point in view
+  int n_cap = 2048;
+  while (n_cap < std::max(std::min(n_map, MF_MAXN), cap) && n_cap < MF_MAXN) n_cap *= 2;
+  MapFilterArgs b;
+  memset(&b, 0, sizeof b);
+  b.keys = keys; b.vis = vis; b.kpts = d_kpts; b.counts = d_counts; b.frames = d_frames; b.T_w_c = d_T_w_c_guess; b.map_pts = d_map_pts;
+  b.batch = batch; b.cap = cap; b.n_map = n_map; b.method = method_index; b.n_cap = n_cap;
+  b.xg_ratio = ctx->prm.xiang_gao_ratio; b.lowe_ratio = ctx->prm.lowe_ratio;
+  b.fx = K[0]; b.fy = K[4]; b.cx = K[2]; b.cy = K[5];
+  b.fcols = (float)cols; b.frows = (float)rows;
+  b.out = d_out; b.cand = d_cand; b.cand_xy = d_cand_xy; b.matches = d_matches; b.p3 = d_pts3d; b.p2 = d_pts2d;
+  const size_t smem = (size_t)n_cap * (4 + 4 + 2 + 2 + 2) + 3 * ((size_t)n_cap / 16 + 2) * 4 + ((size_t)n_cap / 16 + 2) + 64;
+  MVO_CUDA(ctx, cudaFuncSetAttribute(k_map_match_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  KTimer kt(ctx, KC_TRACK);
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)n_jobs, MF_T, smem, 0, k_map_match_filter, b));
+  ctx->launches++;
+  return MVO_OK;
+}

@@ -1,6 +1,7 @@
 // The match-list filter kernels (k_match_filter: thresholds of matchFeatures + removeDuplicatedMatches restated on the device,
-// see the comment in track.cu; k_match_filter_batch: the same body once per frame pair of mvo_match_features_batch_dev) and the
-// projection helper they share with the other tracking kernels — the text nvcc
+// see the comment in track.cu; k_match_filter_batch: the same body once per frame pair of mvo_match_features_batch_dev;
+// k_map_match_filter: once per (frame, guess pose) job of mvo_vo_map_matches_batch_dev) and the projection helpers they share
+// with the other tracking kernels — the text nvcc
 // compiles, in a header so that the CPU test tier can build it for the host (tests/cpp/track_filter_emu.cpp, through
 // tests/cpp/cuda_emu.h).  Included by track.cu inside an anonymous namespace.
 // MVO_DYN_SMEM(type, name) declares the kernel's dynamic shared memory (`extern __shared__ __align__(16) type name[]` for nvcc).
@@ -33,6 +34,18 @@ __device__ __forceinline__ bool project_point(const float *__restrict__ map_pts,
   return !(zc < 0) && (u > 0 && v > 0 && u < fcols && v < frows);
 }
 
+// T_c_w = inv_rigid(T_w_c) (mvo_internal.h) as the 12 values project_point takes: the same products and sums in the same order,
+// each rounded on its own, so that the pose is the host's to the bit whatever the translation unit's contraction setting
+__device__ __forceinline__ Rt12 tcw_of_twc(const double *__restrict__ T) {
+  Rt12 r;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j) r.v[3 * i + j] = T[4 * j + i];
+    r.v[9 + i] = -__dadd_rn(__dadd_rn(__dmul_rn(T[i], T[3]), __dmul_rn(T[4 + i], T[7])), __dmul_rn(T[8 + i], T[11]));
+  }
+  return r;
+}
 
 constexpr int MF_T = 1024;
 constexpr int MF_MAXN = 8192;        // match-list / keypoint capacity of the device path (host path beyond)
@@ -438,3 +451,134 @@ __global__ void __launch_bounds__(MF_T, 1) k_match_filter_batch(FilterBatchArgs 
   if (threadIdx.x == 0) b.n_out[p] = s_info[2] == 0 ? s_info[0] : MVO_ERR_UNSUPPORTED;   // s_info: written by this thread
 }
 
+// The step of poseEstimationPnP_ before solvePnPRansac (vo_pipeline.cpp: pose_estimation_pnp) for a batch of (frame, guess pose)
+// jobs against one map (mvo_vo_map_matches_batch_dev): one CTA per job.  The CTA projects the map with T_c_w of the guess
+// (getMappointsInCurrentView_), runs the filter over the keys of match_batch_kernel<MODE, true> with the in-view flags, and writes
+// the candidate list, the DMatch records and the PnP inputs.  The candidate rows are written only once the filter has finished,
+// so that a job it cannot finish writes its status alone; until then a record's query_idx holds the map index, which is turned
+// into the candidate rank by a binary search of the (increasing) candidate row.
+struct MapFilterArgs {
+  const uint32_t *keys;         // [n_jobs][n_map][W]
+  uint8_t *vis;                 // [n_jobs][n_map] scratch: in-view flags
+  const mvo_keypoint *kpts;     // [batch][cap] (only read for d_pts2d)
+  const int32_t *counts;        // [batch]
+  const int32_t *frames;        // [n_jobs]
+  const double *T_w_c;          // [n_jobs][16]
+  const float *map_pts;         // [n_map][3]
+  int batch, cap, n_map, method, n_cap;
+  double xg_ratio, lowe_ratio;
+  double fx, fy, cx, cy;
+  float fcols, frows;
+  mvo_map_matches_result *out;  // [n_jobs]
+  int32_t *cand;                // [n_jobs][n_map]
+  float *cand_xy;               // [n_jobs][n_map][2] or null
+  mvo_dmatch *matches;          // [n_jobs][cap]
+  float *p3, *p2;               // [n_jobs][cap][3] / [2] or null
+};
+
+__global__ void __launch_bounds__(MF_T, 1) k_map_match_filter(MapFilterArgs b) {
+  MVO_DYN_SMEM(uint8_t, smraw);
+  __shared__ int32_t s_info[24];
+  __shared__ int s_scan[MF_T / 32];
+  // match_filter_run waits again: griddepcontrol.wait returns at once when the predecessor has already been waited for
+  pdl_wait();
+  pdl_launch_dependents();
+  const int j = blockIdx.x, tid = threadIdx.x;
+  const int f = b.frames[j];
+  const double *T = b.T_w_c + (size_t)j * 16;
+  bool bad = f < 0 || f >= b.batch;
+  for (int q = 0; q < 16; ++q) bad = bad || !isfinite(T[q]);
+  if (bad) {
+    if (tid == 0) b.out[j].status = MVO_ERR_INVALID_ARG;
+    return;
+  }
+  const int nk = min(max(b.counts[f], 0), b.cap), nmap = b.n_map, method = b.method;
+  const Rt12 Tcw = tcw_of_twc(T);
+  uint8_t *vis = b.vis + (size_t)j * nmap;
+  // the thread ranges of match_filter_run: every thread reads back only the flags it wrote itself
+  const int per = (nmap + MF_T - 1) / MF_T, q0 = min(tid * per, nmap), q1 = min(q0 + per, nmap);
+  int nv = 0;
+  for (int q = q0; q < q1; ++q) {
+    float2 uv;
+    const bool in = project_point(b.map_pts, q, Tcw, b.fx, b.fy, b.cx, b.cy, b.fcols, b.frows, uv);
+    vis[q] = in ? 1 : 0;
+    nv += in;
+  }
+  int ncand = 0;
+  const int rank0 = block_excl_scan(nv, s_scan, ncand);
+  int np = 0;
+  mvo_dmatch *mo = b.matches + (size_t)j * b.cap;
+  if (ncand > 0 && nk > 0 && !(method == 2 && nk < 2)) {     // match_into skips the matcher otherwise
+    const int W = method == 2 ? 2 : 1;
+    FilterArgs a = {};
+    a.keys = b.keys + (size_t)j * nmap * W;
+    a.vis = vis;
+    a.nmap = nmap; a.nk = nk; a.method = method; a.n_cap = b.n_cap;
+    a.xg_ratio = b.xg_ratio; a.lowe_ratio = b.lowe_ratio;
+    a.info = s_info;
+    const uint32_t *keys = a.keys;
+    const float *map_pts = b.map_pts;
+    float *p3 = b.p3 ? b.p3 + (size_t)j * b.cap * 3 : nullptr, *p2 = b.p2 ? b.p2 + (size_t)j * b.cap * 2 : nullptr;
+    const mvo_keypoint *kp = p2 ? b.kpts + (size_t)f * b.cap : nullptr;
+    match_filter_run<false>(a, smraw, [&](int o, int mi, int t) {
+      // unpack() of match_host.cpp, as k_match_filter_batch writes it; query_idx is the map index until the rank is known
+      const uint32_t d = keys[(size_t)mi * W] >> 16;
+      mvo_dmatch m;
+      m.query_idx = mi;
+      m.train_idx = t;
+      m.img_idx = method == 3 ? -1 : 0;
+      m.distance = method == 3 ? (float)((double)d / 32.0) : (float)d;
+      mo[o] = m;
+      if (p3) {                                             // vo.cpp:293-301
+        p3[3 * o] = map_pts[3 * mi]; p3[3 * o + 1] = map_pts[3 * mi + 1]; p3[3 * o + 2] = map_pts[3 * mi + 2];
+        p2[2 * o] = kp[t].x; p2[2 * o + 1] = kp[t].y;
+      }
+    });
+    __syncthreads();                                        // s_info: written by thread 0 on every way out of the filter
+    if (s_info[2] != 0) {
+      if (tid == 0) b.out[j].status = MVO_ERR_UNSUPPORTED;
+      return;
+    }
+    np = s_info[0];
+  }
+  int32_t *cand = b.cand + (size_t)j * nmap;
+  float *cxy = b.cand_xy ? b.cand_xy + (size_t)j * nmap * 2 : nullptr;
+  int r = rank0;
+  for (int q = q0; q < q1; ++q) {
+    if (!vis[q]) continue;
+    cand[r] = q;
+    if (cxy) {
+      float2 uv;
+      (void)project_point(b.map_pts, q, Tcw, b.fx, b.fy, b.cx, b.cy, b.fcols, b.frows, uv);
+      cxy[2 * r] = uv.x; cxy[2 * r + 1] = uv.y;
+    }
+    ++r;
+  }
+  __syncthreads();                                          // the candidate row, for the ranks
+  for (int o = tid; o < np; o += MF_T) {
+    const int mi = mo[o].query_idx;
+    int lo = 0, hi = ncand;                                 // the first candidate >= mi: mi itself
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (cand[mid] < mi) lo = mid + 1; else hi = mid; }
+    mo[o].query_idx = lo;
+  }
+  if (tid == 0) {
+    mvo_map_matches_result res;
+    res.status = MVO_OK; res.n_candidates = ncand; res.n_matches = np; res.pad = 0;
+    b.out[j] = res;
+  }
+}
+
+// The projected pixels of every map point for every job (mvo_vo_map_matches_batch_dev, method 3: the radius gate of the matcher
+// needs them before the filter has run); grid.y = jobs.  A job with a non-finite pose writes pixels nobody reads.
+__global__ void __launch_bounds__(256) k_project_map_batch(const float *__restrict__ map_pts, int nmap, const double *__restrict__ T_w_c,
+                                                           double fx, double fy, double cx, double cy, float fcols, float frows,
+                                                           float2 *__restrict__ xy) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y;
+  if (i >= nmap) return;
+  const Rt12 Tcw = tcw_of_twc(T_w_c + (size_t)j * 16);
+  float2 uv;
+  (void)project_point(map_pts, i, Tcw, fx, fy, cx, cy, fcols, frows, uv);
+  xy[(size_t)j * nmap + i] = uv;
+}

@@ -45,6 +45,9 @@ KEYFRAME_POINTS_RESULT_DTYPE = np.dtype(
     [("status", "<i4"), ("usable", "<i4"), ("n_matches", "<i4"), ("n_inliers", "<i4"), ("n_kept", "<i4"), ("pad", "<i4"),
      ("median_angle", "<f8"), ("R_curr_to_prev", "<f8", (9,)), ("t_curr_to_prev", "<f8", (3,))])
 assert KEYFRAME_POINTS_RESULT_DTYPE.itemsize == 128
+# mvo_map_matches_result (vo_map_matches_batch_dev): one record per (frame, guess pose) job
+MAP_MATCHES_RESULT_DTYPE = np.dtype([("status", "<i4"), ("n_candidates", "<i4"), ("n_matches", "<i4"), ("pad", "<i4")])
+assert MAP_MATCHES_RESULT_DTYPE.itemsize == 16
 
 MVO_OK = 0
 ERR_NAMES = {0: "MVO_OK", -1: "MVO_ERR_INVALID_ARG", -2: "MVO_ERR_NO_DEVICE", -3: "MVO_ERR_CUDA",
@@ -189,6 +192,8 @@ SIGNATURES = {
                                               _vp]),
     "mvo_vo_keyframe_points_batch_dev": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(VoParams), _vp, _vp,
                                               _vp, _vp, _vp, _vp]),
+    "mvo_vo_map_matches_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp,
+                                          _vp, _vp]),
     "mvo_vo_has_keyframe": (_i, [_vp, _i]),
     "mvo_write_pose_file": (_i, [C.c_char_p, _vp, _i]),
     "mvo_read_pose_file": (_i, [C.c_char_p, _vp, _i, _pi]),
@@ -382,6 +387,19 @@ class Context:
                                                             _ptr(d_matches), _ptr(d_n_matches), _ptr(d_ess), _ptr(d_ess_inliers),
                                                             _ptr(d_T_w_c), _ptr(K), C.byref(vo_params), _ptr(d_out), _ptr(d_kept),
                                                             _ptr(d_kept_pts3d), _ptr(d_kept_angles), _ptr(d_kept_world), _ptr(d_kept_norm)))
+
+    def vo_map_matches_batch_dev(self, d_kpts, d_desc, d_counts, batch, cap, d_frames, d_T_w_c_guess, n_jobs, d_map_pts, d_map_desc, n_map,
+                                 K, rows, cols, method_index, radius, d_out, d_cand, d_matches, d_cand_xy=None, d_pts3d=None, d_pts2d=None):
+        """The state machine's tracking step before PnP (getMappointsInCurrentView_, the match against the map, the 3D-2D pairs)
+        for n_jobs (frame, guess pose) jobs of an orb_extract_batch_dev output against one map of n_map points, all device
+        pointers except K (host 3x3): job j's MAP_MATCHES_RESULT_DTYPE record in d_out[j], its candidates' map indices at
+        d_cand + j * n_map (and pixels at d_cand_xy + j * n_map * 2), its matches at d_matches + j * cap (query_idx = candidate
+        rank) and, when given, the PnP inputs at d_pts3d + j * cap * 3 and d_pts2d + j * cap * 2."""
+        K = _c(K, np.float64)
+        self._chk(self.lib.mvo_vo_map_matches_batch_dev(self.h, _ptr(d_kpts), _ptr(d_desc), _ptr(d_counts), batch, cap, _ptr(d_frames),
+                                                        _ptr(d_T_w_c_guess), n_jobs, _ptr(d_map_pts), _ptr(d_map_desc), n_map, _ptr(K),
+                                                        rows, cols, method_index, C.c_float(radius), _ptr(d_out), _ptr(d_cand),
+                                                        _ptr(d_cand_xy), _ptr(d_matches), _ptr(d_pts3d), _ptr(d_pts2d)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):
