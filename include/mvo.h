@@ -622,7 +622,7 @@ int mvo_vo_keyframe_points_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, c
 /* The first step of the state machine's tracking branch (poseEstimationPnP_) for many frames at once, entirely on the device:
  * for every job (frame, guess pose) what pose_estimation_pnp computes before solvePnPRansac — getMappointsInCurrentView_, the
  * match of the map points in view against the frame (matchFeatures with the tracking method and radius, xiang_gao_ratio /
- * lowe_ratio of the context) and the 3D-2D pairs.  The batched PnP is not part of this call.
+ * lowe_ratio of the context) and the 3D-2D pairs.  The batched PnP that consumes them is mvo_vo_pnp_batch_dev.
  * Inputs: d_kpts / d_desc / d_counts / batch / cap in the layout of mvo_orb_extract_batch_dev; d_frames: n_jobs int32 frame
  * indices; d_T_w_c_guess: n_jobs x 16 doubles, the guess pose of each job (camera->world, row-major; the state machine uses the
  * reference keyframe's pose); d_map_pts / d_map_desc: one map, n_map points (float x, y, z) and descriptors, whose position is
@@ -660,6 +660,39 @@ int mvo_vo_map_matches_batch_dev(mvo_ctx *ctx, const mvo_keypoint *d_kpts, const
                                  const uint8_t *d_map_desc, int n_map, const double *K, int rows, int cols, int method_index,
                                  float radius, mvo_map_matches_result *d_out, int32_t *d_cand, float *d_cand_xy, mvo_dmatch *d_matches,
                                  float *d_pts3d, float *d_pts2d);
+
+/* The rest of poseEstimationPnP_ on the device for every job of a map-matches batch: solvePnPRansac with its least-squares refit,
+ * the inlier matches (matches_with_map_ after the swap), T_w_c = [R|t]^-1 and the jump check against the previous frame.
+ * Inputs: d_mm / d_matches / d_pts3d / d_pts2d / n_jobs / cap exactly as mvo_vo_map_matches_batch_dev wrote them (job j's pairs at
+ * + j * cap); d_T_w_c_prev: n_jobs x 16 doubles, each job's previous-frame pose (prev_->T_w_c_ at PnP time); K: host 3x3; from tp
+ * the call reads min_pnp_points and max_dist_to_prev; the context supplies pnp_hypotheses, pnp_reproj_error, pnp_seed and
+ * pnp_refine_iters (pnp_mode 0 only).
+ * Job j: n_matches < min_pnp_points gives status MVO_OK, pnp_ok 0, no model and T_w_c = T_w_c_prev.  Otherwise the job gets the
+ * consensus set and refit that a single mvo_solve_pnp_ransac call on its pairs returns (the same hypotheses, counts and arg-max;
+ * the refit's sums run in the order of a single device call on cap pairs); no model is not an error (pnp_ok 0).  T_w_c is taken
+ * from Rt without a Rodrigues round trip, and trans_dist(T_w_c, T_w_c_prev) >= max_dist_to_prev (host operation order, no
+ * contraction) rejects the pose: T_w_c = T_w_c_prev.  A rejected job still writes n_inliers and its rows.
+ * Outputs of job j (nothing past a count is written): d_out[j]; d_inliers + j * cap: the consensus set as ascending indices into
+ * the match list (n_inliers); d_kept + j * cap: those matches (optional, NULL: not written).
+ * Per job, status only: the map-matches status when it is not MVO_OK; MVO_ERR_INVALID_ARG for n_matches outside [0, cap] or a
+ * non-finite entry of its T_w_c_prev.
+ * MVO_ERR_INVALID_ARG: a null required pointer (all but d_kept), fx or fy not finite and > 0, cap < 1, n_jobs < 0, a non-finite
+ * max_dist_to_prev.  MVO_ERR_UNSUPPORTED: pnp_mode 1, cap > 8192, n_jobs > 65535, n_jobs * pnp_hypotheses > 2^22.
+ * Asynchronous on the context stream: five kernel launches (hypotheses, scoring, consensus set, refit, record) whatever n_jobs
+ * is, none for n_jobs = 0.  No host synchronisation once the context's scratch has reached its size. */
+typedef struct mvo_vo_pnp_result {
+  int32_t status;     /* MVO_OK, or the job's mvo_status */
+  int32_t pnp_ok;     /* poseEstimationPnP_'s is_pnp_good (mvo_vo_frame_info::pnp_ok) */
+  int32_t n_matches;  /* pairs handed to solvePnPRansac (the map-matches record's n_matches) */
+  int32_t n_inliers;  /* consensus-set size (mvo_vo_frame_info::n_inliers); 0 without a model */
+  int32_t best;       /* winning hypothesis, -1 without a model */
+  int32_t pad[3];
+  double Rt[12];      /* world->camera R (row-major), t after the refit; identity without a model */
+  double T_w_c[16];   /* curr_->T_w_c_ when poseEstimationPnP_ returns (mvo_vo_frame_info::T_w_c_pnp) */
+} mvo_vo_pnp_result;  /* 256 bytes */
+int mvo_vo_pnp_batch_dev(mvo_ctx *ctx, const mvo_map_matches_result *d_mm, const mvo_dmatch *d_matches, const float *d_pts3d,
+                         const float *d_pts2d, int n_jobs, int cap, const double *d_T_w_c_prev, const double *K,
+                         const mvo_track_params *tp, mvo_vo_pnp_result *d_out, int32_t *d_inliers, mvo_dmatch *d_kept /* optional */);
 
 typedef struct mvo_vo_frame_info {
   int32_t frame_id, state_in, state_out;   /* states: 0 BLANK, 1 DOING_INITIALIZATION, 2 DOING_TRACKING (vo.h:52-58) */

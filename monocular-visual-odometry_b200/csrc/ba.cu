@@ -866,10 +866,17 @@ __device__ void pose_pass(const PoseArgs &a, int F, int nchunks, const double *P
   }
 }
 
-template <int CH, bool CACHED, bool STORE>
+// BATCH: one independent LM per cluster (mvo_vo_pnp_batch_dev's refits), job j = cluster index; its edges are rows j * E of
+// e_frame / X / obs, its pose and stats rows j * 12 * F and j * 16.  Each job keeps its own damping and stopping rule.
+template <int CH, bool CACHED, bool STORE, bool BATCH = false>
 __global__ void __launch_bounds__(PF_T, 1) k_ba_pose(PoseArgs a) {
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank(), csize = cluster.num_blocks();
+  if constexpr (BATCH) {
+    const size_t j = blockIdx.x / csize;
+    a.e_frame += j * a.E; a.X += j * a.E * 3; a.obs += j * a.E * 2;
+    a.poses += j * 12 * a.F; a.stats += j * 16;
+  }
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long long t_start = clock64();       // cycles outside the trial loop, debug only (stats 4..7, 12, 13; s_c[3..6] on thread 0)
   pdl_wait();                                // PnP finish / the glue kernel wrote what this kernel reads (launch_pdl.cuh)
@@ -1148,21 +1155,24 @@ static int pose_cluster_size() {
   return (env_cluster >= 1 && env_cluster <= PF_MAXC) ? env_cluster : BA_CLUSTER;
 }
 
-static int pose_launch(mvo_ctx *ctx, void (*kern)(PoseArgs), const PoseArgs &a, int csz, size_t smem) {
+static int pose_launch(mvo_ctx *ctx, void (*kern)(PoseArgs), const PoseArgs &a, int csz, size_t smem, int n_clusters = 1) {
   if (smem > PF_SMEM_MAX) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "pose BA: shared memory %zu B", smem);
   MVO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   {
     KTimer kt(ctx, KC_BA);
-    MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)csz, PF_T, smem, (unsigned)csz, kern, a));      // one cluster; may start under its predecessor's tail
+    // one cluster per LM; may start under its predecessor's tail
+    MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)(n_clusters * csz), PF_T, smem, (unsigned)csz, kern, a));
   }
   ctx->launches++;
   return MVO_OK;
 }
 
-// Launch the pose-only LM on device-resident edge arrays (also used by the PnP refit).
+// Launch the pose-only LM on device-resident edge arrays (also used by the PnP refit).  n_jobs > 0: that many independent one-frame
+// LMs in one launch (chunk 1), job j on rows j * E of the edge arrays, d_poses + 12 j and d_stats + 16 j; each job's sums run in
+// the order of a single launch with the same E.
 int mvo_ba_pose_launch(mvo_ctx *ctx, int F, int E, int chunk, const int32_t *d_eframe, const double *d_X, const double *d_obs, double fx, double fy,
                        double cx, double cy, const double *info, int iters, int use_huber, double huber, int fix_first,
-                       double step_tol, double *d_poses, double *d_stats) {
+                       double step_tol, double *d_poses, double *d_stats, int n_jobs = 0) {
   PoseArgs a;
   memset(&a, 0, sizeof a);
   a.chunk = chunk;
@@ -1174,6 +1184,10 @@ int mvo_ba_pose_launch(mvo_ctx *ctx, int F, int E, int chunk, const int32_t *d_e
   const int csz = pose_cluster_size();
   const bool cached = chunk >= 1 && chunk <= 4 && E / chunk <= csz * PF_T;
   const size_t smem = pose_smem_doubles(F, cached ? chunk : 0, csz) * sizeof(double);
+  if (n_jobs > 0) {
+    if (F != 1 || chunk != 1) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "pose BA batch: one frame and chunk 1 per job");
+    return pose_launch(ctx, cached ? k_ba_pose<1, true, false, true> : k_ba_pose<1, false, false, true>, a, csz, smem, n_jobs);
+  }
   void (*kern)(PoseArgs) = k_ba_pose<1, false, false>;
   if (cached) {
     switch (chunk) {

@@ -184,7 +184,7 @@ void mvo_destroy(mvo_ctx *ctx) {
                    &ctx->orb_cand, &ctx->orb_bandcnt, &ctx->orb_sel, &ctx->orb_misc, &ctx->orb_in,
                    &ctx->orb_kpts, &ctx->orb_desc, &ctx->orb_counts, &ctx->match_part,
                    &ctx->match_tickets, &ctx->match_in, &ctx->match_keys, &ctx->matchb_part, &ctx->matchb_tickets,
-                   &ctx->matchb_keys, &ctx->mapm_buf, &ctx->epib_buf, &ctx->epi_ess_buf, &ctx->epi_homo_buf, &ctx->pnp_pts, &ctx->pnp_hyp,
+                   &ctx->matchb_keys, &ctx->mapm_buf, &ctx->epib_buf, &ctx->pnpb_buf, &ctx->epi_ess_buf, &ctx->epi_homo_buf, &ctx->pnp_pts, &ctx->pnp_hyp,
                    &ctx->pnp_cnt, &ctx->pnp_out, &ctx->ba_buf};
   for (DevBuf *b : dbs)
     if (b->p) cudaFree(b->p);

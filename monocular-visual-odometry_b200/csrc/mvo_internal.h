@@ -121,6 +121,9 @@ struct mvo_ctx {
   // PnP
   DevBuf pnp_pts, pnp_hyp, pnp_cnt, pnp_out;
   int pnp_last_h = 0;
+  // mvo_vo_pnp_batch_dev: hypotheses, counts, finish outputs and refit rows of every job.  Its own block: the tracker holds
+  // device pointers into pnp_* (mvo_pnp_dev_buffers), so those must never grow under it
+  DevBuf pnpb_buf;
   // BA
   DevBuf ba_buf;
 };
@@ -232,6 +235,7 @@ static_assert(offsetof(MvoTrackResultBlock, filter) == 160, "result block layout
 static_assert(offsetof(MvoTrackResultBlock, pose_before_ba) == 256, "result block layout");
 static_assert(offsetof(MvoTrackResultBlock, ba_stats) == 512, "result block layout");
 static_assert(sizeof(MvoTrackResultBlock) == 768, "result block layout");
+static_assert(sizeof(mvo_vo_pnp_result) == 256 && offsetof(mvo_vo_pnp_result, Rt) == 32, "mvo_vo_pnp_result layout");
 
 // track.cu: k_track_glue's argument, passed by value (the field order and types are the kernel's parameter layout)
 struct MvoTrackGlue {

@@ -15,6 +15,8 @@
 //                     damped Gauss-Newton on SE(3) over the inliers (fp64).
 // All arithmetic fp64: the stage is latency-bound (N*H = 8.2e6 reprojections), not FLOP-bound.
 #include <string.h>
+#include <algorithm>
+#include <cmath>
 #include "mvo_internal.h"
 
 namespace {
@@ -22,6 +24,48 @@ namespace {
 #define PNP_DYN_SMEM(type, name) extern __shared__ type name[]
 #include "launch_pdl.cuh"
 #include "pnp_kernels.cuh"
+
+// The rest of poseEstimationPnP_ (vo.cpp:333-380) for every job of mvo_vo_pnp_batch_dev, one CTA per job: the record, the inlier
+// matches (matches_with_map_ after the swap), T_w_c = [R|t]^-1 and the jump check against the previous frame.  The inverse and
+// the distance use __dmul_rn / __dadd_rn in the host's operation order (inv_rigid, trans_dist): no contraction, the host's bits.
+__global__ void __launch_bounds__(128)
+k_pnp_batch_tail(const mvo_map_matches_result *__restrict__ mm, const mvo_dmatch *__restrict__ matches, int cap,
+                 const double *__restrict__ T_prev, double max_dist, const int32_t *__restrict__ job_st,
+                 const double *__restrict__ pose_io, const int32_t *__restrict__ out_i, const int32_t *__restrict__ inl,
+                 mvo_vo_pnp_result *__restrict__ out, mvo_dmatch *__restrict__ kept) {
+  const int j = blockIdx.x, tid = threadIdx.x;
+  pdl_wait();
+  pdl_launch_dependents();
+  mvo_vo_pnp_result *o = out + j;
+  const int st = job_st[j];
+  if (st != MVO_OK) { if (tid == 0) o->status = st; return; }
+  const int ni = out_i[4 * j], best = out_i[4 * j + 1];          // 0 and -1 without a model (also below min_pnp_points)
+  if (kept)
+    for (int k = tid; k < ni; k += blockDim.x) kept[(size_t)j * cap + k] = matches[(size_t)j * cap + inl[(size_t)j * cap + k]];
+  if (tid != 0) return;
+  const double *P = pose_io + (size_t)j * 12, *Tp = T_prev + (size_t)j * 16;
+  double T[16];
+  int ok = best >= 0;
+  if (ok) {
+    for (int i = 0; i < 3; ++i) {
+      for (int c = 0; c < 3; ++c) T[i * 4 + c] = P[c * 3 + i];
+      T[i * 4 + 3] = -__dadd_rn(__dadd_rn(__dmul_rn(P[i], P[9]), __dmul_rn(P[3 + i], P[10])), __dmul_rn(P[6 + i], P[11]));
+    }
+    T[12] = T[13] = T[14] = 0; T[15] = 1;
+    const double dx = __dadd_rn(T[3], -Tp[3]), dy = __dadd_rn(T[7], -Tp[7]), dz = __dadd_rn(T[11], -Tp[11]);
+    if (sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz))) >= max_dist) ok = 0;
+  }
+  if (!ok)
+    for (int q = 0; q < 16; ++q) T[q] = Tp[q];
+  o->status = MVO_OK;
+  o->pnp_ok = ok;
+  o->n_matches = mm[j].n_matches;
+  o->n_inliers = ni;
+  o->best = best;
+  o->pad[0] = o->pad[1] = o->pad[2] = 0;
+  for (int q = 0; q < 12; ++q) o->Rt[q] = P[q];
+  for (int q = 0; q < 16; ++q) o->T_w_c[q] = T[q];
+}
 
 }  // namespace
 
@@ -58,7 +102,7 @@ struct PnpWs { float *p3, *p2; double *poses, *pose_io, *ex, *eo, *stats; int32_
 // ba.cu
 int mvo_ba_pose_launch(mvo_ctx *ctx, int F, int E, int chunk, const int32_t *d_eframe, const double *d_X, const double *d_obs, double fx, double fy,
                        double cx, double cy, const double *info, int iters, int use_huber, double huber, int fix_first,
-                       double step_tol, double *d_poses, double *d_stats);
+                       double step_tol, double *d_poses, double *d_stats, int n_jobs = 0);
 
 static int pnp_ws(mvo_ctx *ctx, int n, int H, PnpWs *w) {
   auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
@@ -111,8 +155,8 @@ static int pnp_enqueue_hypotheses(mvo_ctx *ctx, const PnpWs &w, int n, const Pnp
     return MVO_OK;
   }
   { KTimer kt(ctx, KC_PNP_HYP);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)((H + 127) / 128), 128, 0, 0, k_pnp_hypotheses, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam,
-                           (uint64_t)ctx->prm.pnp_seed, H, w.poses, w.valid)); }
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)((H + 127) / 128), 128, 0, 0, k_pnp_hypotheses<false>, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam,
+                           (uint64_t)ctx->prm.pnp_seed, H, w.poses, w.valid, PnpJobs())); }
   ctx->launches++;
   return MVO_OK;
 }
@@ -132,7 +176,7 @@ static int pnp_score_finish_cv(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam
   k_pnp_score_cv<<<(H + 7) / 8, 256, 0, ctx->stream>>>(w.p3, w.p2, n, n_dev, cam, (float)thr2, H, w.poses, w.valid, w.counts); }
   MVO_CHECK_LAUNCH(ctx);
   { KTimer kt(ctx, KC_PNP_FINISH);
-  k_pnp_finish<<<1, FIN_T, 0, ctx->stream>>>(w.p3, w.p2, n, n_dev, cam, thr2, H, w.poses, w.counts, 2, ctx->prm.pnp_refine_iters,
+  k_pnp_finish<false><<<1, FIN_T, 0, ctx->stream>>>(w.p3, w.p2, n, n_dev, cam, thr2, H, w.poses, w.counts, 2, ctx->prm.pnp_refine_iters,
                                              w.pose_io, w.out_i, w.inl, w.ex, w.eo, w.ef); }
   MVO_CHECK_LAUNCH(ctx);
   ctx->pnp_last_h = H;
@@ -147,15 +191,15 @@ static int pnp_score_finish(mvo_ctx *ctx, const PnpWs &w, int n, const PnpCam &c
   const size_t smem = (size_t)n * 5 * sizeof(float);
   const double thr2 = (double)ctx->prm.pnp_reproj_error * (double)ctx->prm.pnp_reproj_error;
   // the 48 KB default covers static and dynamic shared memory together: k_pnp_score's own s_wmax[8] counts as well
-  if (smem + 8 * sizeof(float) > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_pnp_score, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (smem + 8 * sizeof(float) > 48 * 1024) MVO_CUDA(ctx, cudaFuncSetAttribute(k_pnp_score<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (H + 7) / 8;                                   // one hypothesis per warp while the CTAs of one wave allow it
   if (grid > 4 * ctx->sm_count) grid = 4 * ctx->sm_count;
   { KTimer kt(ctx, KC_PNP_SCORE);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)grid, 256, smem, 0, k_pnp_score, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)grid, 256, smem, 0, k_pnp_score<false>, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
                            (const double *)w.poses, (const int32_t *)w.valid, w.counts)); }
   ctx->launches++;
   { KTimer kt(ctx, KC_PNP_FINISH);
-  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, FIN_T, 0, 0, k_pnp_finish, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, 1, FIN_T, 0, 0, k_pnp_finish<false>, (const float *)w.p3, (const float *)w.p2, n, n_dev, cam, thr2, H,
                            (const double *)w.poses, (const int32_t *)w.counts, 0, (int)ctx->prm.pnp_refine_iters, w.pose_io, w.out_i, w.inl, w.ex, w.eo, w.ef)); }
   ctx->launches++;
   ctx->pnp_last_h = H;
@@ -232,7 +276,81 @@ extern "C" int mvo_test_pnp_dev(mvo_ctx *ctx, const float *pts3d, const float *p
   return MVO_OK;
 }
 
+// Scoring grid of the batch: the CTAs of all jobs together fill about one wave of 4 per SM, and no job gets more CTAs than it has
+// warps of hypotheses.  Every hypothesis is scored by one warp over all of its job's points, so the counts do not depend on it.
+static int pnp_batch_score_grid(const mvo_ctx *ctx, int n_jobs, int H) {
+  const int per_job = (4 * ctx->sm_count + n_jobs - 1) / n_jobs;
+  return std::max(1, std::min((H + 7) / 8, per_job));
+}
+
+// n_jobs x H hypothesis rows at most (96 + 8 bytes each): the bound of the essential-matrix batch
+static const long long PNP_BATCH_MAX_HYP = 1ll << 22;
+
 extern "C" {
+
+int mvo_vo_pnp_batch_dev(mvo_ctx *ctx, const mvo_map_matches_result *d_mm, const mvo_dmatch *d_matches, const float *d_pts3d,
+                         const float *d_pts2d, int n_jobs, int cap, const double *d_T_w_c_prev, const double *K,
+                         const mvo_track_params *tp, mvo_vo_pnp_result *d_out, int32_t *d_inliers, mvo_dmatch *d_kept) {
+  if (!ctx) return MVO_ERR_INVALID_ARG;
+  if (!d_mm || !d_matches || !d_pts3d || !d_pts2d || !d_T_w_c_prev || !K || !tp || !d_out || !d_inliers)
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "pnp batch: null pointer");
+  if (!(std::isfinite(K[0]) && K[0] > 0 && std::isfinite(K[4]) && K[4] > 0))
+    return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "pnp batch: focal lengths must be finite and positive");
+  if (cap < 1 || n_jobs < 0) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "pnp batch: cap %d, n_jobs %d", cap, n_jobs);
+  if (!std::isfinite(tp->max_dist_to_prev)) return mvo_fail(ctx, MVO_ERR_INVALID_ARG, "pnp batch: max_dist_to_prev not finite");
+  if (ctx->prm.pnp_mode == 1) return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "pnp batch: pnp_mode 1 has no batch form");
+  const int H = ctx->prm.pnp_hypotheses;
+  if (cap > 8192 || n_jobs > 65535 || (long long)n_jobs * H > PNP_BATCH_MAX_HYP)
+    return mvo_fail(ctx, MVO_ERR_UNSUPPORTED, "pnp batch: cap %d (<= 8192), n_jobs %d (<= 65535), n_jobs x pnp_hypotheses %lld (<= %lld)",
+                    cap, n_jobs, (long long)n_jobs * H, PNP_BATCH_MAX_HYP);
+  if (n_jobs == 0) return MVO_OK;
+  PnpCam cam;
+  MVO_TRY(pnp_cam(ctx, K, &cam));
+  MVO_CUDA(ctx, cudaSetDevice(ctx->device));
+  // scratch: hypotheses, validity and counts of every job, the finish outputs, the refit's edge rows and stats, job counts/statuses
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t nj = (size_t)n_jobs, nh = nj * H, ne = nj * cap;
+  const size_t o_poses = 0, o_valid = al(o_poses + nh * 96), o_counts = al(o_valid + nh * 4), o_pose = al(o_counts + nh * 4);
+  const size_t o_outi = al(o_pose + nj * 96), o_ex = al(o_outi + nj * 16), o_eo = al(o_ex + ne * 24), o_ef = al(o_eo + ne * 16);
+  const size_t o_stats = al(o_ef + ne * 4), o_n = al(o_stats + nj * 128), o_st = al(o_n + nj * 4), o_end = al(o_st + nj * 4);
+  MVO_TRY(mvo_reserve(ctx, ctx->pnpb_buf, o_end));
+  uint8_t *b = (uint8_t *)ctx->pnpb_buf.p;
+  double *poses = (double *)(b + o_poses), *pose_io = (double *)(b + o_pose), *ex = (double *)(b + o_ex), *eo = (double *)(b + o_eo);
+  double *stats = (double *)(b + o_stats);
+  int32_t *valid = (int32_t *)(b + o_valid), *counts = (int32_t *)(b + o_counts), *out_i = (int32_t *)(b + o_outi);
+  int32_t *ef = (int32_t *)(b + o_ef), *job_n = (int32_t *)(b + o_n), *job_st = (int32_t *)(b + o_st);
+  const double thr2 = (double)ctx->prm.pnp_reproj_error * (double)ctx->prm.pnp_reproj_error;
+  PnpJobs jb;
+  jb.mm = d_mm; jb.T_prev = d_T_w_c_prev; jb.min_pts = tp->min_pnp_points; jb.n = job_n; jb.status = job_st;
+  { KTimer kt(ctx, KC_PNP_HYP);
+  MVO_CUDA(ctx, launch_pdl3(ctx->stream, dim3((unsigned)((H + 127) / 128), (unsigned)n_jobs), dim3(128), 0, k_pnp_hypotheses<true>, d_pts3d,
+                            d_pts2d, cap, (const int32_t *)nullptr, cam, (uint64_t)ctx->prm.pnp_seed, H, poses, valid, jb)); }
+  ctx->launches++;
+  // the job's points in shared memory (20 bytes each); with the kernel's 32 B of static shared memory above the 48 KB default
+  // from cap = 2457 on
+  const size_t smem = (size_t)cap * 5 * sizeof(float);
+  if (smem + 8 * sizeof(float) > 48 * 1024)
+    MVO_CUDA(ctx, cudaFuncSetAttribute(k_pnp_score<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  { KTimer kt(ctx, KC_PNP_SCORE);
+  MVO_CUDA(ctx, launch_pdl3(ctx->stream, dim3((unsigned)pnp_batch_score_grid(ctx, n_jobs, H), (unsigned)n_jobs), dim3(256), smem,
+                            k_pnp_score<true>, d_pts3d, d_pts2d, cap, (const int32_t *)job_n, cam, thr2, H, (const double *)poses,
+                            (const int32_t *)valid, counts)); }
+  ctx->launches++;
+  { KTimer kt(ctx, KC_PNP_FINISH);
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)n_jobs, FIN_T, 0, 0, k_pnp_finish<true>, d_pts3d, d_pts2d, cap, (const int32_t *)job_n, cam,
+                           thr2, H, (const double *)poses, (const int32_t *)counts, 0, (int)ctx->prm.pnp_refine_iters, pose_io, out_i,
+                           d_inliers, ex, eo, ef)); }
+  ctx->launches++;
+  // one cluster per job with E = cap: each refit sums in the order of a single device call on n_upper = cap pairs
+  static const double I2[4] = {1, 0, 0, 1};
+  MVO_TRY(mvo_ba_pose_launch(ctx, 1, cap, 1, ef, ex, eo, cam.fx, cam.fy, cam.cx, cam.cy, I2, ctx->prm.pnp_refine_iters, 0, 1.0, 0, 1e-8,
+                             pose_io, stats, n_jobs));
+  MVO_CUDA(ctx, launch_pdl(ctx->stream, (unsigned)n_jobs, 128, 0, 0, k_pnp_batch_tail, d_mm, d_matches, cap, d_T_w_c_prev,
+                           tp->max_dist_to_prev, (const int32_t *)job_st, (const double *)pose_io, (const int32_t *)out_i,
+                           (const int32_t *)d_inliers, d_out, d_kept));
+  ctx->launches++;
+  return MVO_OK;
+}
 
 int mvo_solve_pnp_ransac(mvo_ctx *ctx, const float *pts3d, const float *pts2d, int n, const double *K,
                          double *rvec, double *tvec, int32_t *inliers, int *n_inliers) {
@@ -308,7 +426,7 @@ int mvo_pnp_refine(mvo_ctx *ctx, const float *pts3d, const float *pts2d, int n, 
   MVO_CUDA(ctx, cudaMemcpyAsync(w.p2, h2, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
   MVO_CUDA(ctx, cudaMemcpyAsync(w.pose_io, h_pose, 96, cudaMemcpyHostToDevice, ctx->stream));
   { KTimer kt(ctx, KC_PNP_FINISH);
-  k_pnp_finish<<<1, FIN_T, 0, ctx->stream>>>(w.p3, w.p2, n, nullptr, cam, 0.0, 0, nullptr, nullptr, 1, ctx->prm.pnp_refine_iters,
+  k_pnp_finish<false><<<1, FIN_T, 0, ctx->stream>>>(w.p3, w.p2, n, nullptr, cam, 0.0, 0, nullptr, nullptr, 1, ctx->prm.pnp_refine_iters,
                                              w.pose_io, w.out_i, w.inl, w.ex, w.eo, w.ef); }
   MVO_CHECK_LAUNCH(ctx);
   MVO_TRY(pnp_refit(ctx, w, n, cam));

@@ -195,12 +195,46 @@ __device__ int p3p(const V3 *X, const V3 *f, Pose *out) {
   return ns;
 }
 
+// The batch form of these kernels (BATCH = true, mvo_vo_pnp_batch_dev) runs one RANSAC per job of a map-matches batch: job j's
+// correspondences are rows j * n of p3 / p2 (n = the batch's cap), its hypotheses and counts rows j * H.  Its count reaches the
+// scoring and finish kernels through n_dev (one entry per job), as the tracker's device count does.
+struct PnpJobs {
+  const mvo_map_matches_result *mm;       // the map-matches records: status and n_matches of every job
+  const double *T_prev;                   // 16 per job: the previous frame's T_w_c
+  int min_pts;                            // mvo_track_params::min_pnp_points
+  int32_t *n, *status;                    // out: the job's effective count and status, written by block (0, j)
+};
+
+// Job j's status and the count its RANSAC runs on: 0 for a failed job (every hypothesis is then invalid) and for one below
+// min_pts (no solvePnPRansac call, vo.cpp:304-311).  Each check comes before anything is read through the value it checks.
+__device__ __forceinline__ void pnp_job_count(const PnpJobs &jb, int j, int cap, int *status, int *count) {
+  const mvo_map_matches_result r = jb.mm[j];
+  int st = r.status, c = 0;
+  if (st == MVO_OK && (r.n_matches < 0 || r.n_matches > cap)) st = MVO_ERR_INVALID_ARG;
+  if (st == MVO_OK)
+    for (int q = 0; q < 16; ++q)
+      if (!isfinite(jb.T_prev[(size_t)j * 16 + q])) st = MVO_ERR_INVALID_ARG;
+  if (st == MVO_OK && r.n_matches >= jb.min_pts) c = r.n_matches;
+  *status = st;
+  *count = c;
+}
+
+template <bool BATCH = false>
 __global__ void __launch_bounds__(128)
 k_pnp_hypotheses(const float *__restrict__ p3, const float *__restrict__ p2, int n, const int32_t *__restrict__ n_dev,
-                 PnpCam cam, uint64_t seed, int H, double *__restrict__ poses, int32_t *__restrict__ valid) {
+                 PnpCam cam, uint64_t seed, int H, double *__restrict__ poses, int32_t *__restrict__ valid, PnpJobs jb = PnpJobs()) {
   const int h = blockIdx.x * blockDim.x + threadIdx.x;
   pdl_wait();                             // the predecessor (match filter) wrote n_dev / p3 / p2
   pdl_launch_dependents();
+  if constexpr (BATCH) {                  // grid (ceil(H / 128), n_jobs); n = cap
+    const int j = blockIdx.y;
+    int st, cnt;
+    pnp_job_count(jb, j, n, &st, &cnt);
+    if (blockIdx.x == 0 && threadIdx.x == 0) { jb.n[j] = cnt; jb.status[j] = st; }
+    p3 += (size_t)j * n * 3; p2 += (size_t)j * n * 2;
+    poses += (size_t)j * H * 12; valid += (size_t)j * H;
+    n = cnt;
+  }
   if (h >= H) return;
   if (n_dev) n = min(n, *n_dev);          // device-resident tracker: the pair count never visited the host
   if (n < 4) { valid[h] = 0; return; }
@@ -251,11 +285,18 @@ k_pnp_hypotheses(const float *__restrict__ p3, const float *__restrict__ p2, int
 // fraction of a percent — so the counts are identical to the all-fp64 kernel this replaces, while the fp64 pipe
 // (64 lanes/clk/SM, division included) no longer bounds the stage.  One hypothesis per warp, points staged once
 // per CTA in shared memory.
+// BATCH: grid (x, n_jobs), job j = blockIdx.y, its correspondences staged in the n (= cap) rows of shared memory.
+template <bool BATCH = false>
 __global__ void __launch_bounds__(256)
 k_pnp_score(const float *__restrict__ p3, const float *__restrict__ p2, int n, const int32_t *__restrict__ n_dev, PnpCam cam,
             double thr2, int H, const double *__restrict__ poses, const int32_t *__restrict__ valid, int32_t *__restrict__ counts) {
   PNP_DYN_SMEM(float, s_pts);      // [n][5]: X Y Z u v
   __shared__ float s_wmax[8];
+  if constexpr (BATCH) {
+    const int j = blockIdx.y;
+    p3 += (size_t)j * n * 3; p2 += (size_t)j * n * 2; n_dev += j;
+    poses += (size_t)j * H * 12; valid += (size_t)j * H; counts += (size_t)j * H;
+  }
   pdl_wait();
   pdl_launch_dependents();
   if (n_dev) n = min(n, *n_dev);
@@ -332,6 +373,8 @@ constexpr int FIN_T = 1024;
 // inlier indices in inl[] and the one-frame edge list (ex, eo, ef) for the pose-only LM refit.
 // mode 0: arg-max + consensus set; mode 1: every point is an inlier, pose_io holds the start pose; mode 2: cv::solvePnPRansac's
 // flow (pnp_cv_kernels.cuh): the model RANSACPointSetRegistrator::run ends with + its consensus set under the float rule.
+// BATCH: one CTA per job (j = blockIdx.x); every row of the job at its offset, out_i 4 and pose_io 12 per job.
+template <bool BATCH = false>
 __global__ void __launch_bounds__(FIN_T)
 k_pnp_finish(const float *__restrict__ p3, const float *__restrict__ p2, int n, const int32_t *__restrict__ n_dev, PnpCam cam,
              double thr2, int H, const double *__restrict__ poses, const int32_t *__restrict__ counts, int mode, int max_iters,
@@ -340,6 +383,13 @@ k_pnp_finish(const float *__restrict__ p3, const float *__restrict__ p2, int n, 
   __shared__ double s_red[32 * 28];
   __shared__ double s_pose[12];
   __shared__ int s_best, s_cnt[32];
+  if constexpr (BATCH) {
+    const int j = blockIdx.x;
+    p3 += (size_t)j * n * 3; p2 += (size_t)j * n * 2; n_dev += j;
+    poses += (size_t)j * H * 12; counts += (size_t)j * H;
+    pose_io += (size_t)j * 12; out_i += (size_t)j * 4; inl += (size_t)j * n;
+    ex += (size_t)j * n * 3; eo += (size_t)j * n * 2; ef += (size_t)j * n;
+  }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int n_upper = n;                 // the refit is launched for this many edge slots
   pdl_wait();

@@ -48,6 +48,11 @@ assert KEYFRAME_POINTS_RESULT_DTYPE.itemsize == 128
 # mvo_map_matches_result (vo_map_matches_batch_dev): one record per (frame, guess pose) job
 MAP_MATCHES_RESULT_DTYPE = np.dtype([("status", "<i4"), ("n_candidates", "<i4"), ("n_matches", "<i4"), ("pad", "<i4")])
 assert MAP_MATCHES_RESULT_DTYPE.itemsize == 16
+# mvo_vo_pnp_result (vo_pnp_batch_dev): one record per map-matches job
+VO_PNP_RESULT_DTYPE = np.dtype(
+    [("status", "<i4"), ("pnp_ok", "<i4"), ("n_matches", "<i4"), ("n_inliers", "<i4"), ("best", "<i4"), ("pad", "<i4", (3,)),
+     ("Rt", "<f8", (12,)), ("T_w_c", "<f8", (16,))])
+assert VO_PNP_RESULT_DTYPE.itemsize == 256
 
 MVO_OK = 0
 ERR_NAMES = {0: "MVO_OK", -1: "MVO_ERR_INVALID_ARG", -2: "MVO_ERR_NO_DEVICE", -3: "MVO_ERR_CUDA",
@@ -194,6 +199,7 @@ SIGNATURES = {
                                               _vp, _vp, _vp, _vp]),
     "mvo_vo_map_matches_batch_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp,
                                           _vp, _vp]),
+    "mvo_vo_pnp_batch_dev": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, C.POINTER(TrackParams), _vp, _vp, _vp]),
     "mvo_vo_has_keyframe": (_i, [_vp, _i]),
     "mvo_write_pose_file": (_i, [C.c_char_p, _vp, _i]),
     "mvo_read_pose_file": (_i, [C.c_char_p, _vp, _i, _pi]),
@@ -400,6 +406,18 @@ class Context:
                                                         _ptr(d_T_w_c_guess), n_jobs, _ptr(d_map_pts), _ptr(d_map_desc), n_map, _ptr(K),
                                                         rows, cols, method_index, C.c_float(radius), _ptr(d_out), _ptr(d_cand),
                                                         _ptr(d_cand_xy), _ptr(d_matches), _ptr(d_pts3d), _ptr(d_pts2d)))
+
+    def vo_pnp_batch_dev(self, d_mm, d_matches, d_pts3d, d_pts2d, n_jobs, cap, d_T_w_c_prev, K, track_params, d_out, d_inliers,
+                         d_kept=None):
+        """The rest of the state machine's poseEstimationPnP_ (solvePnPRansac with its refit, the inlier matches, T_w_c and the
+        jump check) for the n_jobs jobs of a vo_map_matches_batch_dev output (same rows, same cap), all device pointers except K
+        (host 3x3) and track_params (TrackParams: min_pnp_points, max_dist_to_prev): d_T_w_c_prev holds each job's previous-frame
+        pose (16 doubles); job j's VO_PNP_RESULT_DTYPE record lands in d_out[j], its ascending inlier indices at
+        d_inliers + j * cap and, when given, the inlier matches at d_kept + j * cap."""
+        K = _c(K, np.float64)
+        self._chk(self.lib.mvo_vo_pnp_batch_dev(self.h, _ptr(d_mm), _ptr(d_matches), _ptr(d_pts3d), _ptr(d_pts2d), n_jobs, cap,
+                                                _ptr(d_T_w_c_prev), _ptr(K), C.byref(track_params), _ptr(d_out), _ptr(d_inliers),
+                                                _ptr(d_kept)))
 
     # ---- matching ----------------------------------------------------------------------
     def match_hamming_nn(self, d1, d2):
